@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark: causal striped ring flash attention, forward + backward.
 
-Config (BASELINE.json config 1): total sequence 262144, 32 heads, head dim 128, bf16, batch 1, causal,
+Config: total sequence 262144, 32 heads, head dim 128, bf16, batch 1, causal,
 striped layout, sequence sharded over the N GPUs of one box (STRONG scaling: total work is fixed).
 A "step" is one forward + one backward of the ring attention op on synthetic q/k/v (random-init).
 
@@ -11,13 +11,13 @@ A "step" is one forward + one backward of the ring attention op on synthetic q/k
     python bench.py --impl reference     # the unmodified reference from baseline/_ref (Triton + NCCL P2P)
 
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.  The
-q/k/v shards (>= 268 MB each) are larger than the 126 MB L2, so no explicit flush is needed.
+q/k/v shards (>= 268 MB each) are larger than the 50 MB L2 of an H100, so no explicit flush is needed.
 
-Besides the contract fields the JSON line carries: ``roofline_frac`` (value over N x the measured sustained cuBLAS bf16
-rate of MEASURED_PEAKS.json; the NVLink term of the roofline is reported next to it), ``ring_kv_gbps`` (K/V bytes a
+Besides the contract fields the JSON line carries: ``roofline_frac`` (value over N x the dense bf16 rate of the H100 SXM
+data sheet; the NVLink term of the roofline is reported next to it), ``ring_kv_gbps`` (K/V bytes a
 rank pulls in the forward over the time its in-kernel fetchers are active, N > 1), ``check`` (sampled rows of out / dQ /
 dK / dV of one head against a chunked fp32 oracle at the benchmark's own scale) and ``rows`` with the 1 048 576-token
-configuration the metric sentence of BASELINE.json names (fewer steps, same timing rules).
+configuration (fewer steps, same timing rules; skipped when it would not fit the time budget).
 """
 from __future__ import annotations
 
@@ -53,6 +53,9 @@ def parse_args():
                     help="reference arm only: cap the timed steps so that one timed loop stays inside this budget")
     ap.add_argument("--probe-device", type=int, default=None, help=argparse.SUPPRESS)
     ap.add_argument("--fwd-only", action="store_true", help="diagnostic only (not a valid headline number)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write a fixed sample of the last timed step's out / dQ / dK / dV to "
+                         "DIR/<name>.npy (float32) for output-for-output comparison of two builds")
     ap.add_argument("--memory", default="auto", choices=["auto", "gather", "ring"],
                     help="ring_cuda.CONFIG['memory']: 'ring' = per-hop launches against a 2-slot K/V window (O(n/W) "
                          "workspace); 'auto' picks it for K/V slots >= 256 MiB per rank (the headline config at any N)")
@@ -119,8 +122,9 @@ class ClockSampler:
 
 
 def load_peaks() -> dict:
-    """Roofline denominators: the driver's measurement of this pool's B200s, else the profiling recipe's fallback."""
-    peaks = {"bf16_tflops_sustained": 1400.0, "bf16_tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    """Roofline denominators: MEASURED_PEAKS.json when present, else the H100 SXM data sheet (700 W): dense BF16 and
+    HBM3 bandwidth.  The data-sheet rate is a ceiling, not a rate this box was measured to sustain."""
+    peaks = {"bf16_tflops_sustained": 989.0, "bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             m = json.load(f)
@@ -128,7 +132,7 @@ def load_peaks() -> dict:
         peaks["source"] = "MEASURED_PEAKS.json"
     except Exception:  # noqa: BLE001
         pass
-    peaks["nvlink_gbs"] = 770.0  # measured peer-copy rate per direction (B200_PROFILING.md)
+    peaks["nvlink_gbs"] = 450.0  # H100 SXM NVLink 4 data sheet: 900 GB/s total, 450 GB/s per direction
     return peaks
 
 
@@ -277,7 +281,24 @@ def main():
         fwd = 4.0 * B * H * float(S_) * float(S_) * D * 0.5
         return fwd * (1.0 if args.fwd_only else 3.5)
 
-    def measure(S_: int, steps: int, warmup: int, with_e2e: bool, with_check: bool, sample_clocks: bool):
+    def dump_outputs(last: dict, dump_dir: str):
+        """A fixed, seeded sample of token rows (all heads, all of d) of each output of the last timed step, float32."""
+        import numpy as np
+
+        os.makedirs(dump_dir, exist_ok=True)
+        n_rows = next(iter(last.values())).shape[1]
+        gen = torch.Generator().manual_seed(4321)
+        rows = torch.randperm(n_rows, generator=gen)[:min(n_rows, 512)].sort().values
+        suffix = f"_rank{rank}" if world > 1 else ""
+        for name, t in last.items():
+            if t is None:
+                continue
+            sample = t.detach()[:, rows.to(t.device)].float().cpu().numpy()
+            np.save(os.path.join(dump_dir, f"{name}{suffix}.npy"), sample)
+        np.save(os.path.join(dump_dir, f"sample_rows{suffix}.npy"), rows.numpy().astype(np.float64))
+
+    def measure(S_: int, steps: int, warmup: int, with_e2e: bool, with_check: bool, sample_clocks: bool,
+                dump_dir=None):
         """One configuration: device-timed loop (+ e2e loop, + sampled-row check).  Returns a dict (rank 0 prints)."""
         n_ = S_ // world
         torch.cuda.reset_peak_memory_stats(dev)
@@ -291,13 +312,19 @@ def main():
         def call(q_, k_, v_):
             return attn(q_, k_, v_, bucket)
 
-        def step():
+        last = {}  # outputs of the last timed step (--dump-outputs only; nothing is held across steps)
+
+        def step(capture: bool = False):
             out = call(q, k, v)
             if args.fwd_only:
+                if capture:
+                    last["out"] = out
                 return out
             if ref_env:
                 os.environ["DISABLE_MMA_V5"] = "1"  # forward kernels are compiled by now and keep tcgen05
             out.backward(w)
+            if capture:
+                last.update(out=out, dq=q.grad, dk=k.grad, dv=v.grad)
             q.grad = k.grad = v.grad = None
             return out
 
@@ -331,13 +358,16 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         sync()
         e0.record()
-        for _ in range(steps):
-            step()
+        for i in range(steps):
+            step(capture=bool(dump_dir) and i == steps - 1)
         e1.record()
         sync()
         ms = max_over_ranks(e0.elapsed_time(e1))
         clocks = sampler.stop() if (rank == 0 and sample_clocks) else None
         n_launch = launches["count"] - launches_before
+        if dump_dir:
+            dump_outputs(last, dump_dir)
+        last.clear()
 
         flops_per_step = flops_of(S_)
         row = {
@@ -381,10 +411,10 @@ def main():
                 gbps = kv_bytes_fwd / max(window_ns, 1.0)
                 t = torch.tensor([gbps], device=dev, dtype=torch.float64)
                 dist.all_reduce(t, op=dist.ReduceOp.MIN)
-                row["ring_kv_gbps"] = {"value": float(t.item()), "of_nvlink_770": float(t.item()) / peaks["nvlink_gbs"],
+                row["ring_kv_gbps"] = {"value": float(t.item()), "of_nvlink_peak": float(t.item()) / peaks["nvlink_gbs"],
                                        "bytes_per_rank": kv_bytes_fwd,
-                                       "how": "forward K/V bytes pulled per rank / window in which its 148 in-kernel "
-                                              "fetchers were active (globaltimer), min over ranks"}
+                                       "how": "forward K/V bytes pulled per rank / window in which its in-kernel "
+                                              "fetchers (one per SM) were active (globaltimer), min over ranks"}
 
         if hop_window:
             # the 2-slot window is filled by the copy engines: time a standalone pull of the forward's K/V bytes
@@ -404,7 +434,7 @@ def main():
             sync()
             t = torch.tensor([kv_bytes_fwd / (c0.elapsed_time(c1) * 1e6)], device=dev, dtype=torch.float64)
             dist.all_reduce(t, op=dist.ReduceOp.MIN)
-            row["ring_kv_gbps"] = {"value": float(t.item()), "of_nvlink_770": float(t.item()) / peaks["nvlink_gbs"],
+            row["ring_kv_gbps"] = {"value": float(t.item()), "of_nvlink_peak": float(t.item()) / peaks["nvlink_gbs"],
                                    "bytes_per_rank": kv_bytes_fwd,
                                    "how": "copy-engine pull of the forward's K/V slots from every peer (what fills the "
                                           "2-slot window one hop ahead), standalone after the timed loop, min over ranks"}
@@ -507,13 +537,14 @@ def main():
 
     try:
         main_row = measure(S, args.steps, args.warmup, with_e2e=not args.no_e2e,
-                           with_check=(args.check != "off" and args.impl == "ours"), sample_clocks=True)
+                           with_check=(args.check != "off" and args.impl == "ours"), sample_clocks=True,
+                           dump_dir=args.dump_outputs)
     except BaseException as e:  # noqa: BLE001
         if args.impl == "reference":
             unavailable(f"reference failed to run: {type(e).__name__}: {e}")
         raise
 
-    # the 1 048 576-token row of the metric sentence: a couple of steps, skipped when it would not fit the time budget
+    # the 1 048 576-token row: a couple of steps, skipped when it would not fit the time budget
     rows = []
     S1M = 1048576
     if not args.no_1m and S != S1M and not args.fwd_only and S1M % world == 0:
@@ -546,7 +577,7 @@ def main():
             "data": "synthetic q/k/v (random normal), random upstream gradient",
             "impl": args.impl,
             "config": {
-                "model": "causal striped ring flash-attn (BASELINE.json config 1)",
+                "model": "causal striped ring flash-attn",
                 "global_batch": B,
                 "seq_len": S,
                 "heads": H,

@@ -3,11 +3,11 @@
 reference ``tree_attn_decoding.py``; https://arxiv.org/abs/2408.04093).
 
 Every rank keeps ITS slice of the cache for all layers / heads; a decode step sends the (tiny) query to every rank,
-each rank attends to its slice and the partial results are merged — on B200 in ONE kernel launch per rank and step
-(tcgen05 split-KV attention + in-kernel cross-rank merge over NVLink / NVLS), on CPU with two gloo all-reduces.  New
+each rank attends to its slice and the partial results are merged — on the GPU in ONE kernel launch per rank and step
+(split-KV attention + in-kernel cross-rank merge over NVLink / NVLS), on CPU with two gloo all-reduces.  New
 tokens are appended round-robin so that the shards stay balanced.
 
-    # 8 x B200: 32 query / 8 KV heads, 1M cached tokens (131072 per rank), batch 16, bf16 or fp8-e4m3 cache
+    # 8 x H100 (80 GB): 32 query / 8 KV heads, 1M cached tokens (131072 per rank), batch 16, bf16 or fp8-e4m3 cache
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29500 \
         examples/decode_tree_attention.py --context 1048576 --batch 16 --heads 32 --kv-heads 8 --steps 64 [--fp8]
 
@@ -70,7 +70,7 @@ def run(args) -> float:
     dev = torch.device("cuda", torch.cuda.current_device()) if cuda else torch.device("cpu")
     dt = torch.bfloat16 if cuda else torch.float32
     b, h, hk, d = args.batch, args.heads, args.kv_heads, args.dim_head
-    assert not (args.fp8 and not cuda), "the fp8 cache needs the sm_100a kernel"
+    assert not (args.fp8 and not cuda), "the fp8 cache needs the sm_90a kernel"
 
     gen = torch.Generator().manual_seed(args.seed)  # decode-time stream: the same on every rank (queries, new tokens)
 

@@ -6,7 +6,7 @@ the ring (``auto_shard_seq``; striped for causal load balance) and returns the r
 convention of the reference (``ring_attention.py:560-673``).  Parameter gradients are averaged over all ranks with one
 coalesced all-reduce after the backward (what DDP does, without its per-bucket hooks).
 
-    # one 8 x B200 box: one ring of 8, 65536 tokens per sequence (8192 per rank)
+    # one 8 x H100 box: one ring of 8, 65536 tokens per sequence (8192 per rank)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29500 \
         examples/train_ring_transformer.py --seq-len 65536 --dim 1024 --depth 8 --heads 8 --dim-head 128 --steps 50
 

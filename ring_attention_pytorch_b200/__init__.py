@@ -1,5 +1,5 @@
-"""B200-native ring attention: same capabilities and public API as lucidrains/ring-attention-pytorch
-(reference ``ring_attention_pytorch/__init__.py:1-21``), rebuilt around hand-written sm_100a kernels.
+"""Ring attention with the same capabilities and public API as lucidrains/ring-attention-pytorch
+(reference ``ring_attention_pytorch/__init__.py:1-21``), rebuilt around hand-written sm_90a kernels.
 
 Public exports mirror the reference and add the pieces it only exposes through sub-modules.
 """

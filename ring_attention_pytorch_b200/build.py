@@ -1,9 +1,8 @@
-"""In-tree build of the sm_100a extension (``ring_attention_pytorch_b200/_C.so``).
+"""In-tree build of the sm_90a extension (``ring_attention_pytorch_b200/_C.so``).
 
-Kernels (.cu) are compiled straight with nvcc for ``compute_100a/sm_100a`` and never include torch
+Kernels (.cu) are compiled straight with nvcc for ``compute_90a/sm_90a`` and never include torch
 headers, so a kernel edit rebuilds in seconds; only ``bindings.cpp`` sees torch.  The resulting shared
-object is loaded with ``torch.ops.load_library`` and travels with the repository snapshot to the GPU
-box (no JIT cache involved).
+object is loaded with ``torch.ops.load_library`` from the package directory (no JIT cache involved).
 
     python -m ring_attention_pytorch_b200.build          # incremental
     python -m ring_attention_pytorch_b200.build --force  # rebuild everything
@@ -27,19 +26,17 @@ CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 
 CU_SOURCES = [
-    "umma_probe.cu",
-    "attn_fwd_sm100.cu",
-    "attn_bwd_sm100.cu",
-    "attn_bwd_fused_sm100.cu",
-    "tree_decode_sm100.cu",
-    "tree_decode_tc_sm100.cu",
-    "elementwise_sm100.cu",
+    "attn_fwd_sm90.cu",
+    "attn_bwd_sm90.cu",
+    "tree_decode_sm90.cu",
+    "tree_decode_tc_sm90.cu",
+    "elementwise_sm90.cu",
 ]
 CPP_SOURCES = ["tmap.cpp", "symm.cpp"]
 TORCH_CPP_SOURCES = ["bindings.cpp"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -121,7 +118,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
 
     if jobs:
         if verbose:
-            print(f"[build] compiling {len(jobs)} translation unit(s) for sm_100a ...", flush=True)
+            print(f"[build] compiling {len(jobs)} translation unit(s) for sm_90a ...", flush=True)
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(lambda j: _run(j[0], j[1]), jobs))
 

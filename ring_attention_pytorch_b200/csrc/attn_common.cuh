@@ -63,7 +63,7 @@ __device__ __forceinline__ void classify_tile(const MaskCfg& mc, int qlo, int qh
 //
 // Every warp role (TMA producer, MMA issuer, softmax warps) replays the same deterministic sequence of
 // streamed tiles.  Classifying tiles one at a time on a single thread puts ~100 dependent instructions
-// between two tcgen05.mma issues; here the 32 lanes of a warp classify 32 tiles at once and publish the
+// between two MMA issues; here the 32 lanes of a warp classify 32 tiles at once and publish the
 // result as ballot masks, so advancing to the next visible tile is a find-first-set.
 //
 // Sequence order: repeat `groups` times { for hop s in [0, hop_count) { tiles ascending } }.

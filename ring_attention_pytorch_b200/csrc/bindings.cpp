@@ -44,60 +44,6 @@ void check_16bit(const Tensor& t, const char* name) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// descriptor probe
-// ---------------------------------------------------------------------------------------------
-Tensor umma_probe(const Tensor& a, const Tensor& b, int64_t mode, int64_t n, int64_t k, int64_t idesc,
-                  int64_t a_lbo, int64_t a_sbo, int64_t b_lbo, int64_t b_sbo, int64_t b_kstep) {
-  check_16bit(a, "a");
-  check_16bit(b, "b");
-  TORCH_CHECK(a.is_contiguous() && b.is_contiguous());
-  c10::cuda::CUDAGuard guard(a.device());
-  CUtensorMap map_a, map_b;
-  if (mode == 3) {  // a is At [k, 128] (MN-major A); b [k, 64] is written to shared memory by the kernel's threads
-    TORCH_CHECK(a.size(0) == k && a.size(1) == 128 && b.size(0) == k && b.size(1) == 64 && n == 64);
-    uint64_t adims[2] = {128, (uint64_t)k};
-    uint64_t astr[1] = {128 * 2};
-    uint32_t abox[2] = {64, (uint32_t)k};
-    map_a = rab::make_tmap_bf16(a.data_ptr(), 2, adims, astr, abox, rab::TmapSwizzle::B128);
-    map_b = map_a;
-  } else {
-    TORCH_CHECK(a.size(0) == 128 && a.size(1) == k);
-    uint64_t adims[2] = {(uint64_t)k, 128};
-    uint64_t astr[1] = {(uint64_t)k * 2};
-    uint32_t abox[2] = {64, 128};
-    map_a = rab::make_tmap_bf16(a.data_ptr(), 2, adims, astr, abox, rab::TmapSwizzle::B128);
-  }
-  if (mode == 3) {
-  } else if (mode == 0) {
-    TORCH_CHECK(b.size(0) == n && b.size(1) == k);
-    uint64_t bdims[2] = {(uint64_t)k, (uint64_t)n};
-    uint64_t bstr[1] = {(uint64_t)k * 2};
-    uint32_t bbox[2] = {64, (uint32_t)n};
-    map_b = rab::make_tmap_bf16(b.data_ptr(), 2, bdims, bstr, bbox, rab::TmapSwizzle::B128);
-  } else {
-    TORCH_CHECK(b.size(0) == k && b.size(1) == n);
-    uint64_t bdims[2] = {(uint64_t)n, (uint64_t)k};
-    uint64_t bstr[1] = {(uint64_t)n * 2};
-    uint32_t bbox[2] = {64, (uint32_t)k};
-    map_b = rab::make_tmap_bf16(b.data_ptr(), 2, bdims, bstr, bbox, rab::TmapSwizzle::B128);
-  }
-  rab::ProbeParams p;
-  p.mode = (int)mode;
-  p.n = (int)n;
-  p.k = (int)k;
-  p.idesc = (uint32_t)idesc;
-  p.a_lbo = (uint32_t)a_lbo;
-  p.a_sbo = (uint32_t)a_sbo;
-  p.b_lbo = (uint32_t)b_lbo;
-  p.b_sbo = (uint32_t)b_sbo;
-  p.b_kstep_bytes = (uint32_t)b_kstep;
-  Tensor out = torch::empty({128, n}, a.options().dtype(at::kFloat));
-  rab::launch_umma_probe(map_a, map_b, p, mode == 3 ? b.data_ptr() : a.data_ptr(), out.data_ptr<float>(),
-                         at::cuda::getCurrentCUDAStream());
-  return out;
-}
-
-// ---------------------------------------------------------------------------------------------
 // fused ring attention forward
 // ---------------------------------------------------------------------------------------------
 void fill_posmap(rab::PosMap& pm, int64_t stride, int64_t seg_len, at::IntArrayRef base0, at::IntArrayRef base1,
@@ -109,15 +55,6 @@ void fill_posmap(rab::PosMap& pm, int64_t stride, int64_t seg_len, at::IntArrayR
     pm.base0[i] = i < world ? (int)base0[i] : 0;
     pm.base1[i] = i < world ? (int)base1[i] : 0;
   }
-}
-
-// cycles for `reps` back-to-back tcgen05.mma of one flavour on `ctas` SMs: returns [ctas, 2] (total, issue-side)
-Tensor umma_rate(int64_t mode, int64_t n, int64_t reps, int64_t alt, int64_t ctas) {
-  TORCH_CHECK(n == 64 || n == 128 || n == 256, "n must be 64, 128 or 256");
-  Tensor out = torch::zeros({ctas, 2}, torch::dtype(at::kLong).device(at::kCUDA));
-  rab::launch_umma_rate((int)mode, (int)n, (int)reps, (int)alt, (int)ctas,
-                        reinterpret_cast<long long*>(out.data_ptr<int64_t>()), at::cuda::getCurrentCUDAStream());
-  return out;
 }
 
 // Hop mode (memory = "ring"): kv_buf holds ONE owner's slot ([1, 2, b*hk, n_k, d]); the launch visits that owner only
@@ -383,7 +320,7 @@ std::tuple<Tensor, Tensor> attn_bwd_dkdv(const Tensor& qdo_buf, const Tensor& kv
   return {dk, dv};
 }
 
-// One-kernel (5-GEMM) ring backward, head dim 128 (attn_bwd_fused_sm100.cu).
+// One-kernel (5-GEMM) ring backward, head dim 128 (attn_bwd_sm90.cu, KV-stationary kernel in its one-pass form).
 //   qdo [2][b*h][n_q][d] 16 bit and stat [2][b*h][n_pad] fp32: this rank's bwd_prep output
 //   kv_buf [world][2][b*hk][n_k][d]: the K/V gather (slot o valid once ready[o] >= ready_target; no flags: all valid)
 //   dq_acc fp32 [b*h][n_pad][d], zeroed by the caller: dQ (unscaled) is ADDED into it
@@ -460,11 +397,7 @@ std::tuple<Tensor, Tensor> attn_bwd_ring(const Tensor& qdo, const Tensor& kv_buf
   const uint8_t* kv_base = reinterpret_cast<const uint8_t*>(kv_buf.data_ptr()) -
                            (hop_mode ? (size_t)slot_owner * kstr[2] * 2 : 0);  // see attn_fwd_impl
   CUtensorMap map_kv = rab::make_tmap_bf16(kv_base, 4, kdims, kstr, kbox, rab::TmapSwizzle::B128);
-  // dQ accumulator: 2-D (d, b*h*n_pad) fp32, box 32 columns x 32 rows, no swizzle (rows written lane-contiguous)
-  uint64_t adims[2] = {(uint64_t)d, (uint64_t)batch * heads * n_pad};
-  uint64_t astr[1] = {(uint64_t)d * 4};
-  uint32_t abox[2] = {32, 32};
-  CUtensorMap map_dq = rab::make_tmap_f32(dq_acc.data_ptr(), 2, adims, astr, abox, rab::TmapSwizzle::None);
+  p.dq_acc = dq_acc.data_ptr<float>();
 
   Tensor dk, dv;
   if (dkv_acc_ptrs.empty()) {
@@ -478,14 +411,9 @@ std::tuple<Tensor, Tensor> attn_bwd_ring(const Tensor& qdo, const Tensor& kv_buf
     dk = torch::empty({0}, kv_buf.options());
     dv = torch::empty({0}, kv_buf.options());
     p.ring_reduce = 1;
-    uint64_t ddims[2] = {(uint64_t)d, (uint64_t)2 * batch * kv_heads * nk_pad};
-    uint64_t dstr[1] = {(uint64_t)d * 4};
-    uint32_t dbox[2] = {32, 32};
-    for (int o = 0; o < world; ++o)
-      p.map_dkv[o] = rab::make_tmap_f32(reinterpret_cast<const void*>(dkv_acc_ptrs[o]), 2, ddims, dstr, dbox,
-                                        rab::TmapSwizzle::B128);
+    for (int o = 0; o < world; ++o) p.dkv_acc[o] = reinterpret_cast<float*>(dkv_acc_ptrs[o]);
   }
-  rab::launch_attn_bwd_fused(map_qd64, map_kv, map_dq, p, sm_count(), stream);
+  rab::launch_attn_bwd_fused(map_qd64, map_kv, p, sm_count(), stream);
   return {dk, dv};
 }
 
@@ -593,13 +521,14 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   p.eps = (float)eps;
   c10::cuda::CUDAGuard guard(q.device());
   if (tensor_core) {
-    TORCH_CHECK(d == 128 && n > 0, "the tcgen05 decode kernel needs head dim 128 and a non-empty shard");
-    // K, V [b*hk, n, d] -> dims (d, n, b*hk); box = one 128-byte wide, 128-key sub-tile
+    TORCH_CHECK(d == 128 && n > 0, "the tensor-core decode kernel needs head dim 128 and a non-empty shard");
+    // K, V [b*hk, n, d] with any plane stride (a growing cache is read in place) -> dims (d, n, b*hk);
+    // box = one 128-byte wide, 64-key sub-tile
     const uint64_t eb = p.kv_kind == 2 ? 1 : 2;
     uint64_t dims[3] = {(uint64_t)d, (uint64_t)n, (uint64_t)b * kv_heads};
     uint64_t strides[2] = {(uint64_t)d * eb, (uint64_t)kv_plane_stride * eb};
     TORCH_CHECK(strides[1] % 16 == 0, "k / v plane stride must be a multiple of 16 bytes");
-    uint32_t box[3] = {(uint32_t)(128 / eb), 128, 1};
+    uint32_t box[3] = {(uint32_t)(128 / eb), 64, 1};
     auto mk = [&](const void* base) {
       if (p.kv_kind == 2) return rab::make_tmap_u8(base, 3, dims, strides, box, rab::TmapSwizzle::B128);
       if (p.kv_kind == 1) return rab::make_tmap_f16(base, 3, dims, strides, box, rab::TmapSwizzle::B128);
@@ -703,9 +632,6 @@ void symm_close(int64_t ptr) { rab::symm_close(reinterpret_cast<void*>(ptr)); }
 }  // namespace
 
 TORCH_LIBRARY(rab, m) {
-  m.def("umma_rate(int mode, int n, int reps, int alt, int ctas) -> Tensor");
-  m.def("umma_probe(Tensor a, Tensor b, int mode, int n, int k, int idesc, int a_lbo, int a_sbo, int b_lbo, int "
-        "b_sbo, int b_kstep) -> Tensor");
   m.def("attn_fwd(Tensor q, Tensor kv_buf, int[] peer_ptrs, Tensor ready, Tensor? kmask_bits, int kv_heads, int rank, "
         "bool causal, int window, float scale, float softclamp, int pos_stride, int seg_len, int[] base0, int[] "
         "base1, int q_pos_offset, int[] hop_owner) -> (Tensor, Tensor)");
@@ -742,7 +668,6 @@ TORCH_LIBRARY(rab, m) {
 }
 
 TORCH_LIBRARY_IMPL(rab, CUDA, m) {
-  m.impl("umma_probe", &umma_probe);
   m.impl("attn_fwd", &attn_fwd);
   m.impl("attn_fwd_hop", &attn_fwd_hop);
   m.impl("pack_kv", &pack_kv);
@@ -756,7 +681,6 @@ TORCH_LIBRARY_IMPL(rab, CUDA, m) {
 }
 
 TORCH_LIBRARY_IMPL(rab, CompositeExplicitAutograd, m) {
-  m.impl("umma_rate", &umma_rate);
   m.impl("set_fetch_timing", &set_fetch_timing);
   m.impl("device_barrier", &device_barrier);
   m.impl("peer_copy", &peer_copy);

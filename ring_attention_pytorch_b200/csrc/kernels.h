@@ -12,22 +12,6 @@ namespace rab {
 constexpr int kMaxWorld = 16;
 
 // ------------------------------------------------------------------------------------------------
-// descriptor probe (tests)
-// ------------------------------------------------------------------------------------------------
-struct ProbeParams {
-  int mode;  // 0: SS K-major x K-major, 1: SS with MN-major B, 2: TS (A in TMEM) with MN-major B
-  int n;     // MMA N
-  int k;     // reduction length (multiple of 16, <= 128)
-  uint32_t idesc;
-  uint32_t a_lbo, a_sbo;
-  uint32_t b_lbo, b_sbo;
-  uint32_t b_kstep_bytes;  // start-address advance per K=16 step for an MN-major B operand
-};
-void launch_umma_probe(const CUtensorMap& map_a, const CUtensorMap& map_b, const ProbeParams& p,
-                       const void* a_raw, float* out, cudaStream_t stream);
-void launch_umma_rate(int mode, int n, int reps, int alt, int ctas, long long* out, cudaStream_t stream);
-
-// ------------------------------------------------------------------------------------------------
 // position maps: how local index i on ring rank r maps to a global token position.
 //   i <  seg_len : base0[r] + stride * i
 //   i >= seg_len : base1[r] + stride * (i - seg_len)
@@ -122,11 +106,11 @@ void launch_attn_bwd_dkdv(const CUtensorMap& map_qd64, const CUtensorMap& map_kv
                           int num_sms, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
-// one-kernel (5-GEMM) ring backward, head dim 128 (attn_bwd_fused_sm100.cu)
+// one-kernel (5-GEMM) ring backward, head dim 128 (KV-stationary kernel of attn_bwd_sm90.cu in its one-pass form)
 //   local  : qdo [2][b*h][n_q][d] 16 bit, stat [2][b*h][n_pad] fp32 (lse*log2e, delta), dq_acc fp32 [b*h][n_pad][d]
 //   K/V    : gather buffer [world][2][b*hk][n_k][d]; slot o usable once ready[o] >= ready_target (null: always)
 //   dK/dV  : ring_reduce == 0: 16 bit [b, n_k, hk, d] written directly (single rank)
-//            ring_reduce == 1: added into owner o's fp32 [2][b*hk][nk_pad][d] accumulator through map_dkv[o]
+//            ring_reduce == 1: added into owner o's fp32 [2][b*hk][nk_pad][d] accumulator dkv_acc[o] (peer-mapped)
 // ------------------------------------------------------------------------------------------------
 struct AttnBwdFusedParams {
   int batch, heads, kv_heads;
@@ -146,11 +130,12 @@ struct AttnBwdFusedParams {
   uint32_t ready_target;
   void* dk;
   void* dv;
+  float* dq_acc;
   int ring_reduce;
-  alignas(64) CUtensorMap map_dkv[kMaxWorld];
+  float* dkv_acc[kMaxWorld];
 };
-void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const CUtensorMap& map_dq,
-                           const AttnBwdFusedParams& p, int num_sms, cudaStream_t stream);
+void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdFusedParams& p,
+                           int num_sms, cudaStream_t stream);
 size_t attn_bwd_fused_smem_bytes();
 // fp32 accumulator [b*h][n_pad][d] -> 16 bit [b][n][h][d], multiplied by scale
 void launch_acc_convert(const float* acc, void* out, int batch, int heads, int n, int n_pad, int d, float scale,
@@ -163,7 +148,7 @@ void launch_bwd_prep(const void* q, const void* o, const void* dout, const float
                      cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
-// tree-attention decode (tree_decode_sm100.cu): ONE persistent cooperative kernel per rank and step
+// tree-attention decode (tree_decode_sm90.cu): ONE persistent cooperative kernel per rank and step
 // ------------------------------------------------------------------------------------------------
 struct TreeDecodeParams {
   const void* q;            // [b, h, d]; q_kind 0 bf16, 1 fp16, 2 fp32
@@ -193,13 +178,13 @@ struct TreeDecodeParams {
 };
 int tree_decode_max_ctas(int d, int kv_kind, int num_sms);
 void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream);
-// tcgen05 variant (tree_decode_tc_sm100.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 128-key box
+// wgmma variant (tree_decode_tc_sm90.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 64-key box
 int tree_decode_tc_max_ctas(int kv_kind, int num_sms);
 void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, const TreeDecodeParams& p, int grid,
                            cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
-// misc kernels (elementwise_sm100.cu)
+// misc kernels (elementwise_sm90.cu)
 // ------------------------------------------------------------------------------------------------
 // k, v [b, n, hk, d] (arbitrary batch/seq/head strides, unit d stride) -> slot [2][b*hk][n][d]
 // which: bit 0 = pack the K half, bit 1 = pack the V half
@@ -207,7 +192,7 @@ void launch_pack_kv(const void* k, const void* v, void* slot, int batch, int n, 
                     long long k_sb, long long k_sn, long long k_sh, long long v_sb, long long v_sn,
                     long long v_sh, int which, cudaStream_t stream);
 
-// rotary embedding (rotate-half convention) fused with a layout change; see elementwise_sm100.cu:rotary_kernel
+// rotary embedding (rotate-half convention) fused with a layout change; see elementwise_sm90.cu:rotary_kernel
 void launch_rotary(const void* x, void* out, const float* angles, int astride, int batch, int n, int heads, int d,
                    long long sb, long long sn, long long sh, long long ob, long long on, long long oh, float sign,
                    int is_bf16, cudaStream_t stream);

@@ -1,9 +1,8 @@
-// Hand-written sm_100a PTX wrappers: mbarrier, TMA (tensor + bulk), tcgen05 (alloc / mma / commit /
-// ld / st / fences), UMMA shared-memory + instruction descriptors, system-scope flags.
+// Hand-written sm_90a PTX wrappers: mbarrier, TMA (tensor + bulk), wgmma and its shared-memory descriptors,
+// system-scope flags.
 //
-// Everything in here is written against the PTX ISA for sm_100a (CUDA 12.9); no CUTLASS/CuTe types
-// are used.  Descriptor bit layouts follow the hardware definition (the same one CuTe documents in
-// cute/arch/mma_sm100_desc.hpp) and are validated on-device by tests/test_umma_probe.py.
+// Everything in here is written against the PTX ISA for sm_90a (CUDA 12.x); no CUTLASS/CuTe types are used.
+// Descriptor bit layouts follow the hardware definition of the sm_90 matrix descriptor.
 #pragma once
 
 #include <cuda.h>
@@ -92,15 +91,29 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Blocking wait with a watchdog.  `tag` identifies the call site in the trap message.
+// Watchdog report: the block and call-site tag of the watchdog that fired are left in rab_watchdog_info (and printed
+// when RAB_WATCHDOG_PRINTF is 1), then the kernel traps.  printf is a function call, and a call anywhere in a kernel
+// makes ptxas serialize its wgmma (C7510).  The attention kernels keep it: with the serialized schedule they measured
+// faster on H100 (ptxas spills more in the unserialized one).  The decode kernel defines RAB_WATCHDOG_PRINTF 0.
+#ifndef RAB_WATCHDOG_PRINTF
+#define RAB_WATCHDOG_PRINTF 1
+#endif
+static __device__ unsigned long long rab_watchdog_info;
+__device__ __forceinline__ void watchdog_trap(int tag) {
+  *reinterpret_cast<volatile unsigned long long*>(&rab_watchdog_info) =
+      (static_cast<unsigned long long>(blockIdx.x) << 32) | static_cast<uint32_t>(tag);
+#if RAB_WATCHDOG_PRINTF
+  printf("[rab] watchdog: block %d thread %d tag %d\n", (int)blockIdx.x, (int)threadIdx.x, tag);
+#endif
+  __threadfence_system();
+  __trap();
+}
+
+// Blocking wait with a watchdog.  `tag` identifies the call site.
 __device__ __forceinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity, int tag) {
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > RAB_WATCHDOG_CYCLES) {
-      printf("[rab] mbarrier watchdog: block %d thread %d tag %d parity %u\n", (int)blockIdx.x,
-             (int)threadIdx.x, tag, parity);
-      __trap();
-    }
+    if (clock64() - t0 > RAB_WATCHDOG_CYCLES) watchdog_trap(tag);
   }
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
@@ -180,182 +193,236 @@ __device__ __forceinline__ void bulk_wait() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, ld/st, fences
+// wgmma (warpgroup MMA, sm_90a): D[64 x N] fp32 registers (+)= A[64 x 16] . B[16 x N]
+//
+// Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[4j + e] holds
+//   row 16 w + l / 4 + 8 (e / 2),  column 8 j + 2 (l % 4) + (e % 2).
+// A register fragment (16-bit, one K = 16 step): a[0] = (row r, k 2(l%4)..+1), a[1] = (row r + 8, same k),
+// a[2] = (row r, k 8 + 2(l%4)..+1), a[3] = (row r + 8, same k): columns 16 kk .. 16 kk + 15 of an accumulator
+// become the A operand of step kk with no data movement.
+// TA / TB = 1: the operand is MN-major in shared memory (transposed), 16-bit types only.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Keep the compiler from moving accumulator reads / writes across an asynchronous wgmma.
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
+
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Warp-collective variants: every lane of the (converged) warp executes the statement with warp-uniform
-// operands and ONE elected lane issues.  Keeping the call site uniform lets ptxas hold descriptors in uniform
-// registers instead of emitting a per-MMA divergence-safe broadcast loop (profiles/ncu_r1b).
-__device__ __forceinline__ void umma_ss_w(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_ts_w(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_w(uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-// Tell the compiler a value is warp-uniform (it came from shared memory, so ptxas cannot prove it).
-__device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-
-// All previously issued tcgen05.mma of this thread arrive on `bar` when complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d), "n"(TB));
 }
 
-// TMEM -> registers, shape 32x32b: thread t of warp w reads lane 32*(w%4)+t, N consecutive columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3])
-               : "memory");
-}
-// registers -> TMEM, shape 32x32b.
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-      "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-      "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
-// ------------------------------------------------------------------------------------------------
-// UMMA descriptors
-// ------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit):
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, %70;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma16_ss_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TB>
+__device__ __forceinline__ void wgmma16_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma16_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TB>
+__device__ __forceinline__ void wgmma16_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, %70;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n8(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %6, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3}, %4, %5, p, 1, 1, %7, %8;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma16_ss_n8(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %6, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 "
+      "{%0, %1, %2, %3}, %4, %5, p, 1, 1, %7, %8;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma16_ss_n16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <bool BF16, int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  static_assert(N == 8 || N == 16 || N == 64 || N == 128, "wgmma N");
+  if constexpr (N == 8) {
+    if constexpr (BF16) wgmma_ss_n8<TA, TB>(d, a_desc, b_desc, scale_d);
+    else wgmma16_ss_n8<TA, TB>(d, a_desc, b_desc, scale_d);
+  } else if constexpr (N == 16) {
+    if constexpr (BF16) wgmma_ss_n16<TA, TB>(d, a_desc, b_desc, scale_d);
+    else wgmma16_ss_n16<TA, TB>(d, a_desc, b_desc, scale_d);
+  } else if constexpr (N == 64) {
+    if constexpr (BF16) wgmma_ss_n64<TA, TB>(d, a_desc, b_desc, scale_d);
+    else wgmma16_ss_n64<TA, TB>(d, a_desc, b_desc, scale_d);
+  } else {
+    if constexpr (BF16) wgmma_ss_n128<TA, TB>(d, a_desc, b_desc, scale_d);
+    else wgmma16_ss_n128<TA, TB>(d, a_desc, b_desc, scale_d);
+  }
+}
+template <bool BF16, int N, int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  static_assert(N == 64 || N == 128, "wgmma N");
+  if constexpr (N == 64) {
+    if constexpr (BF16) wgmma_rs_n64<TB>(d, a, b_desc, scale_d);
+    else wgmma16_rs_n64<TB>(d, a, b_desc, scale_d);
+  } else {
+    if constexpr (BF16) wgmma_rs_n128<TB>(d, a, b_desc, scale_d);
+    else wgmma16_rs_n128<TB>(d, a, b_desc, scale_d);
+  }
+}
+
+// Shared-memory matrix descriptor (64 bit, sm_90):
 //   [0,14)  start address >> 4          [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4 [46,48) version (1 on sm_100)
-//   [49,52) base offset                 [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
-__host__ __device__ constexpr uint64_t umma_smem_desc_hi_lo(uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                             uint32_t layout_type) {
-  return (uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16) | (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) |
-         (uint64_t(1) << 46) | (uint64_t(layout_type & 7) << 61);
+//   [32,46) stride-dim byte offset >> 4 [49,52) base offset   [62,64) layout: 0 none, 1 = 128B, 2 = 64B, 3 = 32B swizzle
+// 128B-swizzled operands only here.  K-major: 8-row groups SBO = 1024 B apart, LBO unused; the start address advances by
+// 32 B per K = 16 step inside a 128-byte row.  MN-major: LBO = byte distance of consecutive 64-element MN blocks,
+// SBO = 1024 B between 8-row K groups (a K = 16 step advances 2048 B).
+__host__ __device__ constexpr uint64_t gmma_desc_static(uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16) | (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) | (uint64_t(1) << 62);
 }
-__device__ __forceinline__ uint64_t umma_desc(uint64_t static_bits, uint32_t smem_addr) {
-  return static_bits | uint64_t((smem_addr >> 4) & 0x3FFF);
+__device__ __forceinline__ uint64_t gmma_desc(uint64_t static_bits, const void* smem) {
+  return static_bits | uint64_t((smem_u32(smem) >> 4) & 0x3FFF);
 }
-// Advance a descriptor's start address by a byte offset (multiple of 16).  Shared-memory addresses are below
-// 256 KB, so the 14-bit (addr >> 4) field never carries into the neighbouring fields.
-__device__ __forceinline__ uint64_t umma_desc_add(uint64_t desc, uint32_t byte_off) {
-  return desc + uint64_t(byte_off >> 4);
-}
-constexpr uint32_t UMMA_LAYOUT_SW128 = 2;
+// Shared-memory addresses are below 256 KB, so the 14-bit (addr >> 4) field never carries into its neighbour.
+__device__ __forceinline__ uint64_t gmma_desc_add(uint64_t desc, uint32_t byte_off) { return desc + uint64_t(byte_off >> 4); }
 
-// Instruction descriptor (32 bit) for kind::f16 with fp32 accumulate:
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (0 f16, 1 bf16)  [10,13) B fmt  [15] A major (1 = MN)
-//   [16] B major (1 = MN)  [17,23) N >> 3                [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major, uint32_t fmt /*0 f16, 1 bf16*/) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+// Byte offset of 16-bit element (row, col) inside a [rows][64] tile stored with the 128-byte swizzle (1024-B aligned).
+__device__ __forceinline__ uint32_t sw128_off(int row, int col) {
+  return uint32_t(row * 128 + ((((col >> 3) ^ row) & 7) << 4) + ((col & 7) << 1));
+}
+
+// Named barrier over `count` threads (a warpgroup: 128).
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -387,11 +454,7 @@ __device__ __forceinline__ void spin_until_ge_gpu(const uint32_t* p, uint32_t ta
   const long long t0 = clock64();
   while (ld_acquire_gpu(p) < target) {
     __nanosleep(200);
-    if (clock64() - t0 > RAB_WATCHDOG_CYCLES) {
-      printf("[rab] flag watchdog: block %d tag %d have %u want %u\n", (int)blockIdx.x, tag, ld_acquire_gpu(p),
-             target);
-      __trap();
-    }
+    if (clock64() - t0 > RAB_WATCHDOG_CYCLES) watchdog_trap(tag);
   }
 }
 
@@ -417,23 +480,12 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
-// Packed fp32x2 arithmetic (Blackwell FFMA2 / FADD2 / FMUL2): two independent fp32 operations per issue slot.
+// fp32x2 helpers (two independent scalar operations; sm_90 has no packed fp32 instructions).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ua = *reinterpret_cast<unsigned long long*>(&a), ub = *reinterpret_cast<unsigned long long*>(&b),
-                     uc = *reinterpret_cast<unsigned long long*>(&c), ud;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(ud) : "l"(ua), "l"(ub), "l"(uc));
-  return *reinterpret_cast<float2*>(&ud);
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  unsigned long long ua = *reinterpret_cast<unsigned long long*>(&a), ub = *reinterpret_cast<unsigned long long*>(&b), ud;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(ud) : "l"(ua), "l"(ub));
-  return *reinterpret_cast<float2*>(&ud);
-}
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  unsigned long long ua = *reinterpret_cast<unsigned long long*>(&a), ub = *reinterpret_cast<unsigned long long*>(&b), ud;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(ud) : "l"(ua), "l"(ub));
-  return *reinterpret_cast<float2*>(&ud);
-}
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 
 __device__ __forceinline__ void red_add_f32(float* addr, float v) {
   asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
@@ -446,25 +498,6 @@ __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-// 2^x for two values on the FMA pipe: round-to-nearest split x = n + f (magic-number add), degree-3 minimax polynomial
-// for 2^f on [-0.5, 0.5] (relative error 1.2e-4, p(0) == 1 exactly), 2^n added into the exponent field.  Takes a share of
-// the softmax exponentials off the MUFU (16 ex2 / clk / SM, the unit that ties with the tensor core in the forward).
-// -inf (masked logits) returns exactly 0; valid for x < 128.
-__device__ __forceinline__ float2 poly_exp2x2(float2 x) {
-  x.x = fmaxf(x.x, -127.f);
-  x.y = fmaxf(x.y, -127.f);
-  const float2 t = fadd2(x, make_float2(12582912.f, 12582912.f));  // 1.5 * 2^23: low mantissa bits hold n
-  const float2 nf = fadd2(t, make_float2(-12582912.f, -12582912.f));
-  const float2 fr = fadd2(x, make_float2(-nf.x, -nf.y));
-  float2 pl = ffma2(make_float2(0.05536489188671112f, 0.05536489188671112f), fr,
-                    make_float2(0.24221116304397583f, 0.24221116304397583f));
-  pl = ffma2(pl, fr, make_float2(0.6932103037834167f, 0.6932103037834167f));
-  pl = ffma2(pl, fr, make_float2(1.f, 1.f));
-  float2 r;
-  r.x = __uint_as_float(__float_as_uint(pl.x) + (__float_as_uint(t.x) << 23));
-  r.y = __uint_as_float(__float_as_uint(pl.y) + (__float_as_uint(t.y) << 23));
-  return r;
 }
 __device__ __forceinline__ float fast_tanh(float x) {
   float y;

@@ -1,4 +1,4 @@
-// Shared pieces of the tree-decode kernels (CUDA-core split-KV kernel and the tcgen05 kernel): query loads, the
+// Shared pieces of the tree-decode kernels (the CUDA-core split-KV kernel): query loads, the
 // multimem (NVLS) wrappers, the grid barrier, and the cross-rank part of a decode step (publish -> signal -> merge).
 #pragma once
 #include <cuda_bf16.h>
@@ -54,10 +54,7 @@ __device__ __forceinline__ void grid_barrier(uint32_t* count, uint32_t* gen) {
     } else {
       const long long t0 = clock64();
       while (ld_acquire_gpu(gen) == my_gen) {
-        if (clock64() - t0 > RAB_WATCHDOG_CYCLES) {
-          printf("[rab] tree decode grid barrier watchdog: block %d\n", (int)blockIdx.x);
-          __trap();
-        }
+        if (clock64() - t0 > RAB_WATCHDOG_CYCLES) watchdog_trap(1700);
       }
     }
   }
@@ -131,10 +128,7 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
       const uint32_t* mine = p.pads[p.rank] + round * kMaxWorld + tid;
       const long long t0 = clock64();
       while ((int32_t)(ld_acquire_sys(mine) - epoch) < 0) {
-        if (clock64() - t0 > 8 * RAB_WATCHDOG_CYCLES) {
-          printf("[rab] tree decode: rank %d waiting for rank %d round %d epoch %u\n", p.rank, tid, round, epoch);
-          __trap();
-        }
+        if (clock64() - t0 > 8 * RAB_WATCHDOG_CYCLES) watchdog_trap(1710 + round);
       }
     }
     __syncthreads();

@@ -40,13 +40,13 @@ from ring_attention_pytorch_b200.parallel.layout import make_position_map
 from ring_attention_pytorch_b200.utils.validate import typecheck
 
 
-def sm100_kernels_usable(dim_head: int = 64) -> bool:
-    """Default of ``use_cuda_kernel``: the hand-written kernels are sm_100a only and cover head dims up to 128; on any
-    other GPU (or larger heads) the modules fall back to the portable ring op instead of failing at launch."""
+def cuda_kernels_usable(dim_head: int = 64) -> bool:
+    """Default of ``use_cuda_kernel``: the hand-written kernels are built for sm_90a (Hopper) only and cover head dims up
+    to 128; on any other GPU (or larger heads) the modules use the portable ring op instead of failing at launch."""
     if not torch.cuda.is_available() or dim_head > 128:
         return False
     try:
-        return torch.cuda.get_device_capability()[0] == 10
+        return torch.cuda.get_device_capability() == (9, 0)
     except Exception:  # noqa: BLE001
         return False
 
@@ -93,7 +93,7 @@ class RingRotaryEmbedding(Module):
 def apply_rotary_pos_emb(pos: Tensor, t: Tensor, head_dim_first: bool = False) -> Tensor:
     """Rotate feature pairs ``(i, i + d/2)`` of ``t`` ([b, n, h, d], or [b, h, n, d] with ``head_dim_first``) by the
     angles ``pos`` [n, d] (both halves of ``pos`` carry the same d/2 angles).  Same convention as the reference
-    (ring_attention.py:160-172) and as ``csrc/elementwise_sm100.cu::rotary_kernel``; computed in fp32."""
+    (ring_attention.py:160-172) and as ``csrc/elementwise_sm90.cu::rotary_kernel``; computed in fp32."""
     ang = pos if head_dim_first else pos.unsqueeze(1)
     half = t.shape[-1] // 2
     cos, sin = ang.cos(), ang.sin()
@@ -249,7 +249,7 @@ class RingAttention(Module):
         use_cuda_kernel: Optional[bool] = None,
     ):
         super().__init__()
-        use_cuda_kernel = default(use_cuda_kernel, sm100_kernels_usable(dim_head))
+        use_cuda_kernel = default(use_cuda_kernel, cuda_kernels_usable(dim_head))
         assert not (use_cuda_kernel and not torch.cuda.is_available())
         self.use_cuda_kernel = use_cuda_kernel
 
@@ -321,7 +321,7 @@ class RingAttention(Module):
                 self.rotary_embed(torch.arange(n, device=x.device))
         any_cuda_inputs = any(t.is_cuda for t in (q, k, v))
         kernel_path = any_cuda_inputs and self.use_cuda_kernel and not self.force_regular_attn
-        # On the sm_100a path the rotation of q and k happens inside the op's pack kernels (fp32 sincos from the same
+        # On the sm_90a path the rotation of q and k happens inside the op's pack kernels (fp32 sincos from the same
         # angles, fused with the head-major repack): no eager elementwise passes over q and k.
         fuse_rotary = kernel_path and exists(rotary_emb) and self.dim_head % 16 == 0
         if exists(rotary_emb) and not fuse_rotary:
@@ -379,7 +379,7 @@ class RingTransformer(Module):
         ff_chunk_size: Optional[int] = None,
     ):
         super().__init__()
-        use_cuda_kernel = default(use_cuda_kernel, sm100_kernels_usable(dim_head))
+        use_cuda_kernel = default(use_cuda_kernel, cuda_kernels_usable(dim_head))
         self.use_cuda_kernel = use_cuda_kernel
         assert not (use_cuda_kernel and not torch.cuda.is_available())
 

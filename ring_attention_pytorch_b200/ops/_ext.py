@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a extension (``_C.so`` → ``torch.ops.rab.*``).
+"""Loader for the in-tree sm_90a extension (``_C.so`` → ``torch.ops.rab.*``).
 
 The extension is mandatory on a GPU box: if a CUDA device is visible and the shared object cannot be
 loaded we raise instead of silently falling back to eager PyTorch.
@@ -51,7 +51,7 @@ def load(build_if_missing: bool = True) -> bool:
             _error = e
             if torch.cuda.is_available():
                 raise RuntimeError(
-                    f"ring_attention_pytorch_b200: the sm_100a extension {_SO} failed to load on a CUDA machine: {e}"
+                    f"ring_attention_pytorch_b200: the sm_90a extension {_SO} failed to load on a CUDA machine: {e}"
                 ) from e
             return False
     return True
@@ -63,5 +63,5 @@ def is_loaded() -> bool:
 
 def ops():
     if not load():
-        raise RuntimeError(f"sm_100a extension unavailable: {_error}")
+        raise RuntimeError(f"sm_90a extension unavailable: {_error}")
     return torch.ops.rab

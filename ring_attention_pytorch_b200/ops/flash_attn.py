@@ -7,8 +7,8 @@ for the backward.  They exist for users who drive their own hop loop (the refere
 ring_flash_attention_cuda.py:136-186 / 271-337); the ring ops of this package do *not* use them — they run
 every hop inside one kernel and never spill the accumulator.
 
-On a B200 with 16-bit inputs and no bias (or a key-padding bias, the only kind the reference ring op ever
-builds, ring_flash_attention_cuda.py:147-148) one hop is one launch of the sm_100a forward kernel
+On an H100 with 16-bit inputs and no bias (or a key-padding bias, the only kind the reference ring op ever
+builds, ring_flash_attention_cuda.py:147-148) one hop is one launch of the sm_90a forward kernel
 (``torch.ops.rab.attn_fwd``) or of the two backward kernels; the merge of the hop into the carried state is
 the max-rescale identity in fp32.  Everything else (CPU tensors, fp32, arbitrary additive bias matrices)
 takes a dense fp32 PyTorch path with identical semantics, which is also the oracle of the unit tests.

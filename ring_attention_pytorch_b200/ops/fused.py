@@ -1,4 +1,4 @@
-"""Thin Python wrappers over the sm_100a kernels (``torch.ops.rab.*``).
+"""Thin Python wrappers over the sm_90a kernels (``torch.ops.rab.*``).
 
 These are the building blocks the autograd ops in :mod:`ring_attention_pytorch_b200.ops.ring_cuda`
 compose; they are also what the GPU unit tests drive directly.  ``emulate_ring_forward`` runs a whole
@@ -223,7 +223,7 @@ def fused_attn_bwd_ring(
     world: int = 0,
     slot_owner: int = -1,
 ):
-    """The one-kernel (5-GEMM) backward, head dim 128 (``csrc/attn_bwd_fused_sm100.cu``).
+    """The one-kernel (5-GEMM) backward, head dim 128 (``csrc/attn_bwd_sm90.cu``, KV-stationary kernel in its one-pass form).
 
     ``slot_owner >= 0`` (``memory="ring"``): ``kv_buf`` is ONE owner's slot ``[1, 2, b*hk, n_k, d]`` of a ``world``
     rank ring and the launch covers that hop only; ``dq_acc`` and the dK/dV accumulators add up across the launches.

@@ -1,4 +1,4 @@
-"""Ring flash attention on the sm_100a kernels (autograd Function + reference-compatible wrapper).
+"""Ring flash attention on the sm_90a kernels (autograd Function + reference-compatible wrapper).
 
 Public surface mirrors reference ring_flash_attention_cuda.py:353-371 (``ring_flash_attn_cuda`` /
 ``ring_flash_attn_cuda_``) plus a ``layout`` argument ('plain' | 'striped' | 'zigzag').
@@ -7,21 +7,20 @@ Forward, per rank (no host synchronisation, no NCCL on the hot path), ``CONFIG["
 
 ``"ring"`` (what the default ``"auto"`` picks for K/V slots >= 256 MiB per rank) — O(n / W) workspace, like the reference's send/recv ring (ring_flash_attention_cuda.py:128-178):
 
-    pack_kv (K,V -> head-major) into this rank's own SYMMETRIC slot -> device barrier -> one tcgen05 flash-attention
+    pack_kv (K,V -> head-major) into this rank's own SYMMETRIC slot -> device barrier -> one wgmma flash-attention
     launch per ring hop; hop 0 reads the own slot in place, hop s reads a 2-slot window that the COPY ENGINES fill up
     to two hops ahead over NVLink (side stream, events); the un-normalised O / running max / running sum travel between
-    the launches in fp32 buffers (in TMEM inside a launch)
+    the launches in fp32 buffers (in registers inside a launch)
 
 ``"gather"`` (``"auto"`` for short shards) — one launch per rank for the whole ring:
 
     pack_kv straight into this rank's slot of a W-slot symmetric gather workspace -> device barrier -> ONE fused
     kernel: flash attention over every hop while its fetcher warps pull the other ranks' K/V slots over NVLink
-    (bulk TMA) into the local gather buffer; O / max / sum never leave TMEM and registers
+    (bulk TMA) into the local gather buffer; O / max / sum never leave registers
 
-Measured at the headline config (S=262144, h=32, fwd+bwd): same box, back to back, 2 GPUs: 1656 ("ring") vs 1646
-("gather") TFLOP/s, i.e. on par; 8 GPUs: 6369 ("ring") against 6174 ("gather", measured earlier in the round on another
-box, so inside box-to-box variation).  What "ring" buys is memory: S = 4 194 304 on 8 GPUs runs (96 GB per GPU) where the
-W-slot gather alone would need 137 GB.  At short shards the extra launches cost (see ``CONFIG`` below).
+What "ring" buys is memory: its workspace is O(n / W) per rank where the W-slot gather needs O(n).  The two modes
+have not been timed against each other on H100; the threshold between them (``AUTO_RING_SLOT_BYTES``) is a memory
+bound, see ``CONFIG`` below.
 
 Only q, k, v, o and the log-sum-exp are saved for the backward (O(n / W) activation memory per layer; the reference
 saves the same, ring_flash_attention_cuda.py:188-198).  The workspaces are transient and shared by all layers.
@@ -29,8 +28,9 @@ saves the same, ring_flash_attention_cuda.py:188-198).  The workspaces are trans
 Backward, head dim 128 (``CONFIG["backward"] = "fused"``):
 
     bwd_prep (delta, lse -> log2, Q/dO head-major) -> pack_kv into the own slot, zero the fp32 accumulators
-    -> device barrier -> the one-kernel backward (5 GEMMs per tile pair, dQ added into a local fp32 accumulator by TMA
-    reduction, dK/dV tiles added into their OWNER's fp32 accumulators over NVLink from the kernel's epilogue), launched
+    -> device barrier -> the one-kernel backward (5 GEMMs per tile pair, dQ added into a local fp32 accumulator with
+    per-thread vector reductions (red.global.add.v2.f32), dK/dV tiles added the same way into their OWNER's fp32
+    accumulators over NVLink from the kernel's epilogue), launched
     once per hop against the 2-slot window ("ring") or once over the gathered slots, which the copy engines re-pull
     behind per-owner flags ("gather") -> device barrier -> fp32 -> 16 bit
 
@@ -68,20 +68,18 @@ from ring_attention_pytorch_b200.utils.validate import check_attention_inputs, t
 # counts launches of our own kernels (bench.py reports it as gpu_launches)
 LAUNCHES = {"count": 0}
 
-# backward="fused"     : head dim 128 runs the whole backward in ONE KV-stationary kernel (5 GEMMs; dQ through fp32 TMA
-#                        reductions, dK/dV added into the owner's accumulators over NVLink).
+# backward="fused"     : head dim 128 runs the whole backward in ONE KV-stationary kernel (5 GEMMs; dQ through fp32
+#                        vector reductions, dK/dV added into the owner's accumulators over NVLink the same way).
 # backward="two_kernel": the dQ + dK/dV kernel pair (7 GEMMs, no atomics, deterministic); head dim 64 always uses it.
 # memory="ring"        : one launch per ring hop against a 2-slot window that the copy engines fill ahead of the
 #                        kernels; the online-softmax state (forward) and the fp32 accumulators (backward, head dim 128)
-#                        carry over between the launches.  Workspace O(n / W) per rank; on par with "gather" at the
-#                        headline size (see the module docstring).
+#                        carry over between the launches.  Workspace O(n / W) per rank.
 # memory="gather"      : one forward launch per rank; its fetcher warps pull all W-1 peer slots into a W-slot gather
-#                        buffer (transient, shared by all layers); workspace O(n) per rank.  Fewer launches: better for
-#                        short shards, where the one-kernel backward's per-launch ramp shows (8 hops x 8192 keys, h=16:
-#                        726 vs 826 TFLOP/s).  The head-dim-64 / two-kernel backward always gathers.
-# memory="auto"        : "ring" when one rank's K/V slot is at least AUTO_RING_SLOT_BYTES, else "gather".  Measured on 2
-#                        GPUs: 128 MiB slots (S=16384, h=32) ring 1441 vs gather 1546 TFLOP/s — ~90 us of ramp per extra
-#                        launch against 5 ms steps; 2 GiB slots (S=262144) 1656 vs 1646 (same box, back to back).
+#                        buffer (transient, shared by all layers); workspace O(n) per rank.  Fewer launches, which
+#                        favours short shards.  The head-dim-64 / two-kernel backward always gathers.
+# memory="auto"        : "ring" when one rank's K/V slot is at least AUTO_RING_SLOT_BYTES, else "gather".  The threshold
+#                        is a memory bound, not a measured crossover: below it the W-slot gather stays under 4 GiB at
+#                        the largest ring (16 ranks), which fits next to the activations on an 80 GB GPU.
 AUTO_RING_SLOT_BYTES = 256 << 20
 CONFIG = {"backward": "fused", "memory": "auto"}
 
@@ -362,7 +360,7 @@ class RingFlashAttentionCUDAFunction(Function):
             return ready, done
 
         if d_pad == 128 and CONFIG["backward"] == "fused":
-            # ---------------- one-kernel backward (csrc/attn_bwd_fused_sm100.cu) ----------------
+            # ---------------- one-kernel backward (csrc/attn_bwd_sm90.cu, one-pass form) ----------------
             with nvtx_range("rab.bwd.prep"):
                 qdo = alloc_qdo_buffer(1, b, h, n_q, d_pad, dt, dev)
                 stat = alloc_stat_buffer(1, b, h, n_q, dev)
@@ -415,7 +413,7 @@ class RingFlashAttentionCUDAFunction(Function):
                     ops.acc_convert(acc[1], dv, 1.0)
                     _count(3)
         else:
-            # ---------------- two-kernel backward (csrc/attn_bwd_sm100.cu) ----------------
+            # ---------------- two-kernel backward (csrc/attn_bwd_sm90.cu) ----------------
             qdo_gather = alloc_qdo_buffer(ring_size, b, h, n_q, d_pad, dt, dev)
             stat_gather = alloc_stat_buffer(ring_size, b, h, n_q, dev)
             ops.bwd_prep(qp, o, dop, lse, qdo_gather, stat_gather, rank)

@@ -1,7 +1,7 @@
 """Portable ring flash attention (pure PyTorch autograd Function, CPU/gloo or any device).
 
-This is the semantic specification of the framework and the path ``BASELINE.json`` config 0 runs on
-(no GPU).  Capability parity with reference ring_flash_attention.py:60-406, re-derived around position
+This is the semantic specification of the framework and the path that runs without a GPU
+(CPU or any device).  Capability parity with reference ring_flash_attention.py:60-406, re-derived around position
 maps instead of bucket bookkeeping:
 
 * one code path for plain, striped and zig-zag layouts (visibility = ``pos_q >= pos_k``);

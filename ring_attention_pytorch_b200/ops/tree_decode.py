@@ -3,7 +3,7 @@
 
 Layout is head-first like the reference: ``q [b, h, 1, d]``, ``k [b, hk, n, d]``, ``v [b, hk, n, dv]``.
 
-* CUDA path: ``csrc/tree_decode_sm100.cu`` – ONE persistent cooperative kernel per rank and step computes the
+* CUDA path: ``csrc/tree_decode_tc_sm90.cu`` (head dim 128) / ``csrc/tree_decode_sm90.cu`` – ONE persistent cooperative kernel per rank and step computes the
   split-KV partials of its KV shard, merges the splits, publishes ``(out, lse)`` in symmetric memory, signals the
   peers and merges all ranks' partials in-kernel (NVLink peer loads, or ``multimem.ld_reduce`` through the NVSwitch
   when the buffers have a multicast mapping), replacing the reference's Triton launch padded to a 128-row tile plus
@@ -55,7 +55,7 @@ def tree_attn_decode(
     ``shard_kv_seq=True``: every rank passes the *full* K/V and attends to its own ``chunk(world)`` slice
     (ranks beyond the number of chunks contribute nothing).  ``shard_kv_seq=False``: K/V are already this
     rank's shard (``None`` for an empty shard).  ``use_triton`` is kept for signature parity and selects the
-    sm_100a kernel (default: on CUDA inputs).
+    sm_90a kernel (default: on CUDA inputs).
     """
     assert not (exists(k) ^ exists(v)), "keys and values are either both None, or both present"
     dtype = q.dtype
@@ -71,7 +71,7 @@ def tree_attn_decode(
     assert exists(dim_v), "dim_v is required when this rank holds no keys"
 
     use_kernel = default(use_triton, q.is_cuda)
-    assert not (use_kernel and not q.is_cuda), "input needs to be on cuda to use the sm_100a kernel"
+    assert not (use_kernel and not q.is_cuda), "input needs to be on cuda to use the sm_90a kernel"
 
     if use_kernel:
         from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda

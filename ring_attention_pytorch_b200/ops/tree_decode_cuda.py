@@ -1,4 +1,5 @@
-"""sm_100a tree-attention decode: ONE persistent cooperative kernel per rank and step (``csrc/tree_decode_sm100.cu``).
+"""sm_90a tree-attention decode: ONE persistent cooperative kernel per rank and step (``csrc/tree_decode_tc_sm90.cu``,
+``csrc/tree_decode_sm90.cu``).
 
 The kernel computes the split-KV partials of this rank's shard, merges the splits, publishes ``(out, lse)`` in a
 symmetric buffer, signals the peers and merges all ranks' partials — over NVLink peer loads, or, when the buffers have a
@@ -21,8 +22,8 @@ from ring_attention_pytorch_b200.parallel.distributed import get_rank, get_world
 
 LAUNCHES = {"count": 0}
 # nvls "auto": use the NVSwitch multicast mapping when torch's symmetric memory can provide one, else NVLink peer loads
-# tensor_core "auto": head dim 128 shards of at least one 128-key tile run the tcgen05 kernel (K / V tiles go from TMA
-#                     straight into the MMA; fp8 caches use kind::f8f6f4), everything else the CUDA-core kernel
+# tensor_core "auto": head dim 128 runs the wgmma kernel (K / V tiles go from TMA straight into the MMA, read in place
+#                     from the cache; an fp8 cache is widened to bf16 in shared memory), everything else the CUDA-core kernel
 CONFIG = {"nvls": "auto", "tensor_core": "auto"}
 K_MAX_WORLD = 16
 PAD_WORDS = 2 * K_MAX_WORLD  # two signal rounds
@@ -175,11 +176,10 @@ def tree_decode_cuda(
     g = h // hk
     kv_kind = 0 if k is None or k.dtype == torch.bfloat16 else (1 if k.dtype == torch.float16 else 2)
     tc = CONFIG["tensor_core"]
-    # a 128-key tile of the tensor-core kernel must lie inside one scale block
-    use_tc = tc in ("auto", True, "on") and d == 128 and n >= 128 and scale_block_keys % 128 == 0
+    use_tc = tc in ("auto", True, "on") and d == 128 and n >= 1
     if k is not None and not (use_tc and _is_cache_prefix(k) and v.stride() == k.stride()):
         k, v = k.contiguous(), v.contiguous()  # no-op for dense inputs
-    gm = (4 if g <= 4 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: template bound GM)
+    gm = (8 if g <= 8 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: MMA N)
     groups = b * hk * ((g + gm - 1) // gm)
     resident = int(ops.tree_decode_max_ctas(d, kv_kind, use_tc))
     splits = _choose_splits(n, groups, resident)

@@ -2,7 +2,7 @@
 
 A *layout* says which global token position local index ``i`` on ring rank ``r`` holds.  Every layout
 the reference supports is a piecewise-affine map with at most two segments, which is exactly what the
-sm_100a kernels evaluate in registers (``csrc/attn_common.cuh``):
+sm_90a kernels evaluate in registers (``csrc/attn_common.cuh``):
 
     i <  seg_len : base0[r] + stride * i
     i >= seg_len : base1[r] + stride * (i - seg_len)

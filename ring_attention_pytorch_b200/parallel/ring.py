@@ -1,6 +1,6 @@
-"""Host-driven P2P ring for the portable (CPU / gloo, or NCCL without the sm_100a kernels) path.
+"""Host-driven P2P ring for the portable (CPU / gloo, or NCCL without the sm_90a kernels) path.
 
-The sm_100a path never touches this module: there the ring is a *schedule* evaluated inside the kernels
+The sm_90a path never touches this module: there the ring is a *schedule* evaluated inside the kernels
 (``layout.ring_hop_owners`` -> ``hop_owner[]``) and K/V move with in-kernel bulk-TMA copies over NVLink.  The
 portable path follows the same schedule — hop ``s`` of ring rank ``r`` holds the data of owner ``(r - s) mod W`` —
 and realises it by actually rotating the tensors with point-to-point messages, so both backends share one definition

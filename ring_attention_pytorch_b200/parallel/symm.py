@@ -4,10 +4,10 @@ Every rank of a ring set allocates identically sized device regions through the 
 (``csrc/symm.cpp`` – cudaMalloc + CUDA IPC handles), exchanges the 64-byte handles once over
 ``torch.distributed`` and maps every peer's region.  After that the hot path never touches NCCL:
 
-* kernels read peer K/V slots with bulk-TMA copies over NVLink (``attn_fwd_sm100.cu`` fetch warp);
+* kernels read peer K/V slots with bulk-TMA copies over NVLink (``attn_fwd_sm90.cu`` fetch warp);
 * copy engines pull peer Q/dO/stat slots on a side stream in the backward;
 * ranks synchronise with a device-side barrier on peer-mapped signal pads
-  (``elementwise_sm100.cu:device_barrier_kernel``, ``st.release.sys`` / ``ld.acquire.sys``).
+  (``elementwise_sm90.cu:device_barrier_kernel``, ``st.release.sys`` / ``ld.acquire.sys``).
 
 The reference does all of this with ``batch_isend_irecv`` + ``dist.barrier()`` per hop (ring.py:51-60).
 """

@@ -1,7 +1,7 @@
 """Runtime argument validation for the public constructors and ops.
 
 The reference type-checks every public entry point with ``beartype`` (ring_attention.py:47, 103, 284, 489;
-ring_flash_attention.py:391).  ``typecheck`` is that decorator when beartype is importable (it is in the B200 image and
+ring_flash_attention.py:391).  ``typecheck`` is that decorator when beartype is importable (it is a declared dependency and
 listed in ``requirements.txt``) and a no-op otherwise, so the package stays importable on a bare PyTorch install.  On top
 of the annotation checks, ``check_attention_inputs`` validates what annotations cannot express: tensor ranks, matching
 batch / head-dim sizes, grouped-query divisibility and mask shapes — failing with a message that names the argument

@@ -1,6 +1,6 @@
 """Packaging for ring_attention_pytorch_b200 (counterpart of the reference's setup.py:1-31).
 
-``pip install -e .`` / ``python setup.py build_ext --inplace`` compile ``csrc/`` for sm_100a with the in-tree
+``pip install -e .`` / ``python setup.py build_ext --inplace`` compile ``csrc/`` for sm_90a with the in-tree
 builder (``ring_attention_pytorch_b200/build.py``: nvcc per .cu, g++ for the runtime, one ``_C.so`` next to the
 package) — the same artefact ``__graft_entry__.build()`` and the test-suite use, so there is exactly one build path.
 """
@@ -34,7 +34,7 @@ class build_py(_build_py):
 
 
 class build_native(Command):
-    description = "compile the sm_100a extension in-tree"
+    description = "compile the sm_90a extension in-tree"
     user_options = []
 
     def initialize_options(self):
@@ -50,7 +50,7 @@ class build_native(Command):
 setup(
     name="ring-attention-pytorch-b200",
     version="0.1.0",
-    description="B200-native (sm_100a tcgen05/TMEM/TMA + NVLink) ring attention, striped / zig-zag context "
+    description="Hopper-native (sm_90a wgmma/TMA + NVLink) ring attention, striped / zig-zag context "
                 "parallelism and tree-attention decoding",
     packages=find_packages(include=["ring_attention_pytorch_b200", "ring_attention_pytorch_b200.*"]),
     package_data={"ring_attention_pytorch_b200": ["_C.so", "csrc/*"]},

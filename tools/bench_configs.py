@@ -1,4 +1,4 @@
-"""Secondary benchmarks for the other BASELINE.json configs (run under torchrun for N > 1):
+"""Secondary benchmarks (run under torchrun for N > 1):
 
     zigzag   GQA Llama-style heads=32 kv_heads=8, total seq 1 048 576, zig-zag schedule, fwd (+bwd with --bwd)
     decode   tree_attn_decode, 8192 keys per rank, batch 256, 32/8 heads, d=128, bf16 and fp8-e4m3 KV
@@ -97,7 +97,7 @@ def bench_decode(world, rank, dev, n_per_rank, batch, iters):
         from ring_attention_pytorch_b200.ops import tree_decode_cuda as tdc
 
         emit(rank, bench="tree_decode", kv_dtype=name, n_gpus=world, keys_per_rank=n_per_rank, batch=batch, ms=ms,
-             local_kv_gb_per_s=kv_bytes / ms / 1e6, hbm_frac_of_measured_6585=kv_bytes / ms / 1e6 / 6585.0,
+             local_kv_gb_per_s=kv_bytes / ms / 1e6, hbm_frac_of_datasheet_3350=kv_bytes / ms / 1e6 / 3350.0,
              tokens_per_s=batch / (ms * 1e-3), launches_per_step=1, merge="nvls multimem" if tdc.uses_nvls(q) else "nvlink peer loads",
              nvls_unavailable_because=tdc._alloc_symmetric.last_error)
 

@@ -1,18 +1,18 @@
 """Peer K/V fetch micro-benchmark: what do the forward kernel's in-kernel fetchers sustain over NVLink?
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29512 \
-        tools/bench_fetch.py --slot-mb 512 --out profiles/peer_fetch_n2.json
+        tools/bench_fetch.py --slot-mb 512 --out peer_fetch_n2.json
 
 The fused forward is launched with a NEGLIGIBLE attention problem (128 queries, one head) against large K/V slots, so
-the kernel's duration is the transfer: every one of the 148 CTAs' fetcher warps moves its 1/148 share of every remote
+the kernel's duration is the transfer: every CTA's fetcher warp (one CTA per SM) moves its share of every remote
 slot (peer global -> shared memory -> local global, two 16 KB bulk-TMA copies in flight per SM).  Reported per rank:
 
 * ``gbps_window``  bytes pulled / the window between the first fetcher starting and the last one finishing
                    (``%globaltimer``, recorded by the kernel itself)
 * ``gbps_kernel``  bytes pulled / CUDA-event duration of the whole launch
 
-against the measured peer-copy rate (770 GB/s per direction) and the nominal 900 GB/s of NVLink 5.  Also times a
-``cudaMemcpyAsync`` peer pull of the same bytes (the copy-engine path the backward uses) for comparison.
+against the copy-engine rate of the same run and the 450 GB/s per direction of the H100 SXM NVLink 4 data sheet.  The
+copy-engine rate comes from a ``cudaMemcpyAsync`` peer pull of the same bytes (the path the backward uses).
 """
 from __future__ import annotations
 
@@ -103,9 +103,9 @@ def main():
     if rank == 0:
         res = {"n_gpus": world, "slot_mb": args.slot_mb, "bytes_pulled_per_rank": pulled, "per_rank": allr,
                "min_gbps_window": min(a["gbps_window"] for a in allr),
-               "of_measured_770": min(a["gbps_window"] for a in allr) / 770.0,
-               "of_nominal_900": min(a["gbps_window"] for a in allr) / 900.0,
-               "how": "fused forward with negligible attention work; in-kernel globaltimer window of the 148 fetchers"}
+               "of_copy_engine": min(a["gbps_window"] for a in allr) / min(a["gbps_copy_engine"] for a in allr),
+               "of_datasheet_450": min(a["gbps_window"] for a in allr) / 450.0,
+               "how": "fused forward with negligible attention work; in-kernel globaltimer window of the fetchers (one per SM)"}
         print(json.dumps(res))
         if args.out:
             os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

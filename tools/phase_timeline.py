@@ -1,7 +1,7 @@
 """Per-phase CUDA-event timeline of the ring attention op on every rank (run under torchrun).
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 \
-        tools/phase_timeline.py --seq-len 262144 --out profiles/phase_timeline_n8.json
+        tools/phase_timeline.py --seq-len 262144 --out phase_timeline_n8.json
 
 Phases are the ``nvtx_range`` regions of ``ops/ring_cuda.py`` (pack + device barrier, forward kernel, backward prep,
 accumulator zero + barrier, backward kernel + dQ convert, final barrier + dK/dV convert).  Every rank reports the

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Config-5 sweep with the reference beside it (run on a GPU box; N = number of GPUs, default 2):
-#   tools/sweep_vs_reference.sh 2 > profiles/sweep_vs_reference_n2.jsonl
+#   tools/sweep_vs_reference.sh 2 > sweep_vs_reference_n2.jsonl
 # Every line is bench.py's JSON line (ours and --impl reference, same metric / config / timing rules) for one total
 # sequence length; the reference is lucidrains/ring-attention-pytorch's own Triton kernels + NCCL batch_isend_irecv ring
 # (ring.py:51-60) from baseline/_ref, unmodified.
