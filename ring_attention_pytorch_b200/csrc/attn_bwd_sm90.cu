@@ -88,9 +88,11 @@ __device__ __forceinline__ void dq_decode(const AttnBwdParams& p, int idx, DqIte
   it.qhi += p.q_pos_offset;
 }
 
-using DqScan = WarpTileScan<2, false>;
+template <bool DOCS>
+using DqScan = WarpTileScan<2, false, DOCS>;
 
-__device__ __forceinline__ void dq_init_scan(DqScan& sc, const AttnBwdParams& p, const DqItem& it) {
+template <bool DOCS>
+__device__ __forceinline__ void dq_init_scan(DqScan<DOCS>& sc, const AttnBwdParams& p, const DqItem& it) {
   sc.pm = &p.pos;
   sc.hop_owner = p.hop_owner;
   sc.hop_count = p.hop_count;
@@ -111,10 +113,15 @@ __device__ __forceinline__ void dq_init_scan(DqScan& sc, const AttnBwdParams& p,
       hi += p.q_pos_offset;
     }
     sc.st[t] = StatRange{lo, hi, valid, false};
+    if constexpr (DOCS) {
+      if (valid)
+        sc.doc[t] = doc_range(doc_row_spans(p.doc_spans, p.batch, p.n_q, p.rank, it.b), a, min(a + 64, p.n_q) - 1,
+                                 lane_id());
+    }
   }
 }
 
-template <int D>
+template <int D, bool DOCS>
 __device__ __forceinline__ void dq_producer(DqSmem<D>& sm, const AttnBwdParams& p, const CUtensorMap* map_qd,
                                             const CUtensorMap* map_kv) {
   constexpr int NSUB = DqSmem<D>::NSUB;
@@ -136,8 +143,8 @@ __device__ __forceinline__ void dq_producer(DqSmem<D>& sm, const AttnBwdParams& 
                     p.rank * 2 + 1);
       }
     }
-    DqScan scan;
-    dq_init_scan(scan, p, it);
+    DqScan<DOCS> scan;
+    dq_init_scan<DOCS>(scan, p, it);
     ScanTile t;
     while (scan.next(lane, t)) {
       if (lane == 0) {
@@ -160,7 +167,7 @@ __device__ __forceinline__ void dq_producer(DqSmem<D>& sm, const AttnBwdParams& 
 }
 
 // Thread layout as in the forward: rows r_lo and r_lo + 8 of the warpgroup's 64 query rows, column pairs 8 j + cq.
-template <int D, bool BF16>
+template <int D, bool BF16, bool DOCS>
 __device__ __forceinline__ void dq_consumer(DqSmem<D>& sm, const AttnBwdParams& p, const int W) {
   constexpr uint64_t mnmaj = gmma_desc_static(SUB128, 1024);  // K as the MN-major B of dQ += dS K
   const int wg_tid = threadIdx.x - 128 * W;
@@ -190,6 +197,13 @@ __device__ __forceinline__ void dq_consumer(DqSmem<D>& sm, const AttnBwdParams& 
       lse2[h] = row_ok[h] ? p.stat[stat_row + grow[h]] : INFINITY;
       delta[h] = row_ok[h] ? p.stat[stat_row + (size_t)p.batch * p.heads * p.n_pad + grow[h]] : 0.f;
     }
+    int2 span[2];  // document interval of each of this thread's query rows
+    if constexpr (DOCS) {
+      const int2* rows = doc_row_spans(p.doc_spans, p.batch, p.n_q, p.rank, it.b);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) span[h] = rows[min(grow[h], p.n_q - 1)];
+    }
+
     mbar_wait(&sm.qdo_full, n_item & 1, 600 + W);
     const uint64_t q_desc = gmma_desc(KMAJ, sm.q + W * SUB64);
     const uint64_t do_desc = gmma_desc(KMAJ, sm.dout + W * SUB64);
@@ -198,8 +212,8 @@ __device__ __forceinline__ void dq_consumer(DqSmem<D>& sm, const AttnBwdParams& 
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
 
-    DqScan scan;
-    dq_init_scan(scan, p, it);
+    DqScan<DOCS> scan;
+    dq_init_scan<DOCS>(scan, p, it);
     ScanTile t;
     while (scan.next(lane, t)) {
       const uint32_t st = n_tile % DQ_NST, ph = (n_tile / DQ_NST) & 1;
@@ -264,6 +278,7 @@ __device__ __forceinline__ void dq_consumer(DqSmem<D>& sm, const AttnBwdParams& 
                   keep = keep && (pk <= pos_q[h]);
                   if (p.window > 0) keep = keep && (pos_q[h] - pk <= p.window);
                 }
+                if constexpr (DOCS) keep = keep && (span[h].x <= pk) && (pk < span[h].y);
                 if (!keep) pj = 0.f;
               }
               ds2[e] = pj * (dp[i + e] - delta[h]) * chain;
@@ -300,7 +315,7 @@ __device__ __forceinline__ void dq_consumer(DqSmem<D>& sm, const AttnBwdParams& 
   }
 }
 
-template <int D, bool BF16>
+template <int D, bool BF16, bool DOCS>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qd, const __grid_constant__ CUtensorMap map_kv,
                    const __grid_constant__ AttnBwdParams p) {
@@ -319,10 +334,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qd, const __grid_cons
   __syncthreads();
   if (warp >= 8) {
     setmaxnreg_dec<40>();
-    if (warp == 8) dq_producer<D>(sm, p, &map_qd, &map_kv);
+    if (warp == 8) dq_producer<D, DOCS>(sm, p, &map_qd, &map_kv);
   } else {
     setmaxnreg_inc<232>();
-    dq_consumer<D, BF16>(sm, p, warp < 4 ? 0 : 1);
+    dq_consumer<D, BF16, DOCS>(sm, p, warp < 4 ? 0 : 1);
   }
 }
 
@@ -388,11 +403,12 @@ __device__ __forceinline__ void dkv_decode(const P& p, int L, DkvItem& it) {
   it.k_tail = (it.key0 + 128) > p.n_k;
 }
 
-using DkvScan = WarpTileScan<1, true>;
+template <bool DOCS>
+using DkvScan = WarpTileScan<1, true, DOCS>;
 
 // streamed side = query tiles of 64 rows (one-pass: the local queries only); rep = query head inside the GQA group
-template <bool ONE_PASS, class P>
-__device__ __forceinline__ void dkv_init_scan(DkvScan& sc, const P& p, const DkvItem& it) {
+template <bool ONE_PASS, bool DOCS, class P>
+__device__ __forceinline__ void dkv_init_scan(DkvScan<DOCS>& sc, const P& p, const DkvItem& it) {
   sc.pm = &p.pos;
   if constexpr (ONE_PASS) {
     sc.hop_owner = p.self_owner;
@@ -408,9 +424,12 @@ __device__ __forceinline__ void dkv_init_scan(DkvScan& sc, const P& p, const Dkv
   sc.stat_off = 0;
   sc.mc = MaskCfg{p.causal, p.window, p.kmask_bits != nullptr};
   sc.st[0] = StatRange{it.klo, it.khi, true, it.k_tail};
+  if constexpr (DOCS)
+    sc.doc[0] = doc_range(doc_row_spans(p.doc_spans, p.batch, p.n_k, it.owner, it.b), it.key0,
+                             min(it.key0 + 128, p.n_k) - 1, lane_id());
 }
 
-template <int D, bool ONE_PASS, class P>
+template <int D, bool ONE_PASS, bool DOCS, class P>
 __device__ __forceinline__ void dkv_producer(DkvSmem<D>& sm, const P& p, const CUtensorMap* map_qd64,
                                              const CUtensorMap* map_kv) {
   constexpr int NSUB = DkvSmem<D>::NSUB;
@@ -435,8 +454,8 @@ __device__ __forceinline__ void dkv_producer(DkvSmem<D>& sm, const P& p, const C
                     it.owner * 2 + 1);
       }
     }
-    DkvScan scan;
-    dkv_init_scan<ONE_PASS>(scan, p, it);
+    DkvScan<DOCS> scan;
+    dkv_init_scan<ONE_PASS, DOCS>(scan, p, it);
     ScanTile t;
     while (scan.next(lane, t)) {
       if (lane == 0) {
@@ -463,7 +482,7 @@ __device__ __forceinline__ void dkv_producer(DkvSmem<D>& sm, const P& p, const C
 }
 
 // Thread layout: rows (keys) r_lo and r_lo + 8 of the warpgroup's 64 keys, query columns 8 j + cq (+1).
-template <int D, bool BF16, bool ONE_PASS, class P>
+template <int D, bool BF16, bool ONE_PASS, bool DOCS, class P>
 __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const int W) {
   constexpr uint64_t qmn = gmma_desc_static(SUB64, 1024);   // Q / dO as MN-major B (K = queries, N = d)
   constexpr uint64_t kmn = gmma_desc_static(SUB128, 1024);  // K as MN-major B of dQ = dS K (K = keys, N = d)
@@ -495,6 +514,13 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
         key_ok[h] = (wbits >> (key[h] & 31)) & 1u;
       }
     }
+    int2 span[2];  // document interval of each of this thread's keys
+    if constexpr (DOCS) {
+      const int2* rows = doc_row_spans(p.doc_spans, p.batch, p.n_k, it.owner, it.b);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) span[h] = rows[min(key[h], p.n_k - 1)];
+    }
+
     mbar_wait(&sm.kv_full, n_item & 1, 900 + W);
     const uint64_t k_desc = gmma_desc(KMAJ, sm.k + W * SUB64);
     const uint64_t v_desc = gmma_desc(KMAJ, sm.v + W * SUB64);
@@ -503,8 +529,8 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
 
-    DkvScan scan;
-    dkv_init_scan<ONE_PASS>(scan, p, it);
+    DkvScan<DOCS> scan;
+    dkv_init_scan<ONE_PASS, DOCS>(scan, p, it);
     ScanTile t;
     bool any = false;
     while (scan.next(lane, t)) {
@@ -566,6 +592,7 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
               keep = keep && (pos_k[h] <= pq);
               if (p.window > 0) keep = keep && (pq - pos_k[h] <= p.window);
             }
+            if constexpr (DOCS) keep = keep && (span[h].x <= pq) && (pq < span[h].y);
             if (!keep) pj = 0.f;
           }
           pp[e] = pj;
@@ -672,7 +699,7 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
   }
 }
 
-template <int D, bool BF16, bool ONE_PASS, class P>
+template <int D, bool BF16, bool ONE_PASS, bool DOCS, class P>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap map_qd64, const __grid_constant__ CUtensorMap map_kv,
                     const __grid_constant__ P p) {
@@ -691,10 +718,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap map_qd64, const __grid_c
   __syncthreads();
   if (warp >= 8) {
     setmaxnreg_dec<40>();
-    if (warp == 8) dkv_producer<D, ONE_PASS>(sm, p, &map_qd64, &map_kv);
+    if (warp == 8) dkv_producer<D, ONE_PASS, DOCS>(sm, p, &map_qd64, &map_kv);
   } else {
     setmaxnreg_inc<232>();
-    dkv_consumer<D, BF16, ONE_PASS>(sm, p, warp < 4 ? 0 : 1);
+    dkv_consumer<D, BF16, ONE_PASS, DOCS>(sm, p, warp < 4 ? 0 : 1);
   }
 }
 
@@ -788,7 +815,9 @@ template <int D>
 void launch_attn_bwd_dq(const CUtensorMap& map_qd, const CUtensorMap& map_kv, const AttnBwdParams& p, int num_sms,
                         cudaStream_t stream) {
   using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnBwdParams);
-  Kern kern = p.is_bf16 ? attn_bwd_dq_kernel<D, true> : attn_bwd_dq_kernel<D, false>;
+  Kern kern = p.doc_spans != nullptr
+                  ? (p.is_bf16 ? attn_bwd_dq_kernel<D, true, true> : attn_bwd_dq_kernel<D, false, true>)
+                  : (p.is_bf16 ? attn_bwd_dq_kernel<D, true, false> : attn_bwd_dq_kernel<D, false, false>);
   const size_t smem = sizeof(DqSmem<D>) + 1024;
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "bwd_dq smem attr");
   const int items = p.batch * p.heads * ((p.n_q + 127) / 128);
@@ -801,8 +830,10 @@ template <int D>
 void launch_attn_bwd_dkdv(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdParams& p,
                           int num_sms, cudaStream_t stream) {
   using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnBwdParams);
-  Kern kern = p.is_bf16 ? attn_bwd_dkv_kernel<D, true, false, AttnBwdParams>
-                        : attn_bwd_dkv_kernel<D, false, false, AttnBwdParams>;
+  Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_bwd_dkv_kernel<D, true, false, true, AttnBwdParams>
+                                                   : attn_bwd_dkv_kernel<D, false, false, true, AttnBwdParams>)
+                                     : (p.is_bf16 ? attn_bwd_dkv_kernel<D, true, false, false, AttnBwdParams>
+                                                   : attn_bwd_dkv_kernel<D, false, false, false, AttnBwdParams>);
   const size_t smem = sizeof(DkvSmem<D>) + 1024;
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
              "bwd_dkdv smem attr");
@@ -815,8 +846,10 @@ void launch_attn_bwd_dkdv(const CUtensorMap& map_qd64, const CUtensorMap& map_kv
 void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdFusedParams& p,
                            int num_sms, cudaStream_t stream) {
   using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnBwdFusedParams);
-  Kern kern = p.is_bf16 ? attn_bwd_dkv_kernel<128, true, true, AttnBwdFusedParams>
-                        : attn_bwd_dkv_kernel<128, false, true, AttnBwdFusedParams>;
+  Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_bwd_dkv_kernel<128, true, true, true, AttnBwdFusedParams>
+                                                   : attn_bwd_dkv_kernel<128, false, true, true, AttnBwdFusedParams>)
+                                     : (p.is_bf16 ? attn_bwd_dkv_kernel<128, true, true, false, AttnBwdFusedParams>
+                                                   : attn_bwd_dkv_kernel<128, false, true, false, AttnBwdFusedParams>);
   const size_t smem = sizeof(DkvSmem<128>) + 1024;
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "bwd_fused smem attr");
   const int items = p.hop_count * p.batch * p.kv_heads * ((p.n_k + 127) / 128);

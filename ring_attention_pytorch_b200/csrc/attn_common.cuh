@@ -1,6 +1,8 @@
 // Shared device-side helpers for the attention kernels: position maps, tile classification and the
 // deterministic per-work-item KV tile schedule that every warp role replays independently.
 #pragma once
+#include <climits>
+
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -59,6 +61,45 @@ __device__ __forceinline__ void classify_tile(const MaskCfg& mc, int qlo, int qh
 }
 
 // ------------------------------------------------------------------------------------------------
+// Document masking (packed sequences).  spans: int32 [world][batch][n][2], the half-open interval
+// [start, end) of global positions of the document holding local token i of ring rank r (built by
+// parallel/documents.py).  q and k share a document iff pos(k) lies in q's interval iff pos(q) lies in
+// k's, so a kernel only needs the intervals of its stationary rows.
+// ------------------------------------------------------------------------------------------------
+struct DocRange {
+  int min_s, max_s;  // min / max document start over the stationary tile's rows
+  int min_e, max_e;  // min / max document end
+};
+
+__device__ __forceinline__ const int2* doc_row_spans(const int* spans, int batch, int n, int r, int b) {
+  return reinterpret_cast<const int2*>(spans) + ((size_t)r * batch + b) * n;
+}
+
+// Summary of the intervals of rows [a, last] (inclusive).  All 32 lanes call it convergently.
+__device__ __forceinline__ DocRange doc_range(const int2* rows, int a, int last, int lane) {
+  int mn_s = INT_MAX, mx_s = INT_MIN, mn_e = INT_MAX, mx_e = INT_MIN;
+  for (int i = a + lane; i <= last; i += 32) {
+    const int2 s = rows[i];
+    mn_s = min(mn_s, s.x);
+    mx_s = max(mx_s, s.x);
+    mn_e = min(mn_e, s.y);
+    mx_e = max(mx_e, s.y);
+  }
+  return DocRange{__reduce_min_sync(0xffffffffu, mn_s), __reduce_max_sync(0xffffffffu, mx_s),
+                  __reduce_min_sync(0xffffffffu, mn_e), __reduce_max_sync(0xffffffffu, mx_e)};
+}
+
+// Streamed positions [lo, hi] against the stationary rows' intervals: skip when no row's document can reach the
+// range, per-element masking unless every row's document covers all of it.
+__device__ __forceinline__ void classify_doc(const DocRange& d, int lo, int hi, bool& need, bool& partial) {
+  if (hi < d.min_s || lo >= d.max_e) {
+    need = false;
+  } else if (!(d.max_s <= lo && hi < d.min_e)) {
+    partial = true;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Warp-cooperative tile scanner.
 //
 // Every warp role (TMA producer, MMA issuer, softmax warps) replays the same deterministic sequence of
@@ -68,12 +109,21 @@ __device__ __forceinline__ void classify_tile(const MaskCfg& mc, int qlo, int qh
 //
 // Sequence order: repeat `groups` times { for hop s in [0, hop_count) { tiles ascending } }.
 // All 32 lanes must call next() convergently; the scanner state is warp-uniform.
+// DOCS: the stationary tiles also carry a DocRange (doc[i]) and streamed tiles are classified against it.
 // ------------------------------------------------------------------------------------------------
 struct StatRange {
   int lo, hi;   // position range of the stationary tile
   bool valid;   // false: the stationary tile does not exist (e.g. second Q tile beyond n_q)
   bool tail;    // the stationary tile is ragged (forces per-element masking)
 };
+
+// Document summaries of the stationary tiles; empty (and so absent from the default scanners) without documents.
+template <int NSTAT, bool DOCS>
+struct ScanDocs {
+  DocRange doc[NSTAT];
+};
+template <int NSTAT>
+struct ScanDocs<NSTAT, false> {};
 
 struct ScanTile {
   int rep;       // group repetition index
@@ -83,8 +133,8 @@ struct ScanTile {
   bool part[2];
 };
 
-template <int NSTAT, bool STREAM_IS_Q>
-struct WarpTileScan {
+template <int NSTAT, bool STREAM_IS_Q, bool DOCS = false>
+struct WarpTileScan : ScanDocs<NSTAT, DOCS> {
   const PosMap* pm;
   const int* hop_owner;
   int hop_count, groups;
@@ -118,6 +168,7 @@ struct WarpTileScan {
           } else {
             classify_tile(mc, st[i].lo + stat_off, st[i].hi + stat_off, lo, hi, tail || st[i].tail, nd[i], pt[i]);
           }
+          if constexpr (DOCS) classify_doc(this->doc[i], lo, hi, nd[i], pt[i]);
         }
       }
     }

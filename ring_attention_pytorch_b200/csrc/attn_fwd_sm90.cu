@@ -15,9 +15,9 @@
 // The ring itself is only a schedule: ring rank r visits owners hop_owner[0..hop_count) (itself first).
 // K/V of owner o live in slot o of a symmetric [world][2][b*hk][n][d] buffer.  Slot r is written locally
 // by pack_kv; the other slots are filled inside this kernel by the fetcher warps of all CTAs (each moves
-// 1/gridDim of every slot), overlapping the NVLink transfer with the MMAs of earlier hops.  Layout
-// (plain / striped / zig-zag), causal + sliding-window masking and key padding are position functions
-// evaluated in-kernel; fully masked tiles are never loaded.
+// 1/gridDim of every slot), overlapping the NVLink transfer with the MMAs of earlier hops.  Layout (plain / striped /
+// zig-zag), causal + sliding-window masking, key padding and packed documents are position functions evaluated
+// in-kernel; fully masked tiles are never loaded.
 #include <cstdlib>
 
 #include "attn_common.cuh"
@@ -82,9 +82,11 @@ __device__ __forceinline__ void decode_item(const AttnFwdParams& p, int idx, Ite
   }
 }
 
-using FwdScan = WarpTileScan<2, false>;
+template <bool DOCS>
+using FwdScan = WarpTileScan<2, false, DOCS>;
 
-__device__ __forceinline__ void init_scan(FwdScan& sc, const AttnFwdParams& p, const Item& it) {
+template <bool DOCS>
+__device__ __forceinline__ void init_scan(FwdScan<DOCS>& sc, const AttnFwdParams& p, const Item& it) {
   sc.pm = &p.pos;
   sc.hop_owner = p.hop_owner;
   sc.hop_count = p.hop_count;
@@ -96,12 +98,18 @@ __device__ __forceinline__ void init_scan(FwdScan& sc, const AttnFwdParams& p, c
   sc.mc = MaskCfg{p.causal, p.window, p.kmask_bits != nullptr};
 #pragma unroll
   for (int t = 0; t < 2; ++t) sc.st[t] = StatRange{it.qlo[t], it.qhi[t], it.tvalid[t], false};
+  if constexpr (DOCS) {
+    const int2* rows = doc_row_spans(p.doc_spans, p.batch, p.n_q, p.rank, it.b);
+#pragma unroll
+    for (int t = 0; t < 2; ++t)
+      if (it.tvalid[t]) sc.doc[t] = doc_range(rows, it.row0[t], min(it.row0[t] + BM, p.n_q) - 1, lane_id());
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
 // warp 8: TMA producer (all 32 lanes scan tiles, lane 0 issues)
 // ------------------------------------------------------------------------------------------------
-template <int D>
+template <int D, bool DOCS>
 __device__ __forceinline__ void producer_role(FwdSmem<D>& sm, const AttnFwdParams& p, const CUtensorMap* map_q,
                                               const CUtensorMap* map_kv) {
   constexpr int NSUB = FwdSmem<D>::NSUB;
@@ -123,8 +131,8 @@ __device__ __forceinline__ void producer_role(FwdSmem<D>& sm, const AttnFwdParam
         tma_load_4d(sm.q[buf] + s * SUB_BYTES, map_q, &sm.q_full[buf], s * 64, it.h, it.row0[0], it.b);
     }
     items++;
-    FwdScan scan;
-    init_scan(scan, p, it);
+    FwdScan<DOCS> scan;
+    init_scan<DOCS>(scan, p, it);
     ScanTile ti;
     while (scan.next(lane, ti)) {
       if (!((ready_mask >> ti.owner) & 1u)) {
@@ -216,7 +224,7 @@ __device__ __forceinline__ void fetch_role(FwdSmem<D>& sm, const AttnFwdParams& 
 // Every consumer walks the whole tile sequence of the item (also tiles its rows do not need, and items whose second
 // tile lies beyond n_q) so that each K/V stage is released by both warpgroups exactly once, in order.
 // ------------------------------------------------------------------------------------------------
-template <int D, bool BF16>
+template <int D, bool BF16, bool DOCS>
 __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParams& p, const int t) {
   constexpr int NO = D / 2;  // O accumulator registers per thread
   // K-major operands (Q, K): 8-row groups 1024 B apart.  MN-major V (B of P V): d sub-tiles SUB_BYTES apart.
@@ -254,6 +262,12 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
       row_ok[h] = tvalid && grow[h] < p.n_q;
       pos_q[h] = pos_of(p.pos, p.rank, min(grow[h], p.n_q - 1)) + p.q_pos_offset;
     }
+    int2 span[2];  // document interval of each of this thread's rows
+    if constexpr (DOCS) {
+      const int2* rows = doc_row_spans(p.doc_spans, p.batch, p.n_q, p.rank, it.b);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) span[h] = rows[min(grow[h], p.n_q - 1)];
+    }
 
     float o[NO];
     float m_used[2] = {-INFINITY, -INFINITY};
@@ -279,8 +293,8 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
     }
 
     const uint64_t q_desc = gmma_desc(kmaj, sm.q[buf] + t * BM * 128);
-    FwdScan scan;
-    init_scan(scan, p, it);
+    FwdScan<DOCS> scan;
+    init_scan<DOCS>(scan, p, it);
     ScanTile ti;
     while (scan.next(lane, ti)) {
       const bool need = t ? ti.need[1] : ti.need[0];
@@ -333,6 +347,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
               keep = keep && (pk <= pos_q[h]);
               if (p.window > 0) keep = keep && (pos_q[h] - pk <= p.window);
             }
+            if constexpr (DOCS) keep = keep && (span[h].x <= pk) && (pk < span[h].y);
             if (!keep) s[i] = -INFINITY;
           }
         }
@@ -431,7 +446,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
   }
 }
 
-template <int D, bool BF16>
+template <int D, bool BF16, bool DOCS>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
                 const __grid_constant__ AttnFwdParams p) {
@@ -461,13 +476,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   if (warp >= 8) {
     setmaxnreg_dec<40>();
     if (warp == 8) {
-      producer_role<D>(sm, p, &map_q, &map_kv);
+      producer_role<D, DOCS>(sm, p, &map_q, &map_kv);
     } else if (warp == 10) {
       if (lane_id() == 0) fetch_role<D>(sm, p);
     }
   } else {
     setmaxnreg_inc<232>();
-    consumer_role<D, BF16>(sm, p, warp < 4 ? 0 : 1);
+    consumer_role<D, BF16, DOCS>(sm, p, warp < 4 ? 0 : 1);
   }
 }
 
@@ -481,7 +496,9 @@ template <int D>
 void launch_attn_fwd(const CUtensorMap& map_q, const CUtensorMap& map_kv, const AttnFwdParams& p, int num_sms,
                      cudaStream_t stream) {
   using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnFwdParams);
-  const Kern kern = p.is_bf16 ? attn_fwd_kernel<D, true> : attn_fwd_kernel<D, false>;
+  // documents are a separate instantiation: the default kernels keep their code unchanged
+  const Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_fwd_kernel<D, true, true> : attn_fwd_kernel<D, false, true>)
+                                           : (p.is_bf16 ? attn_fwd_kernel<D, true, false> : attn_fwd_kernel<D, false, false>);
   const size_t smem = sizeof(FwdSmem<D>) + 1024;
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
              "attn_fwd smem attribute");

@@ -57,6 +57,18 @@ void fill_posmap(rab::PosMap& pm, int64_t stride, int64_t seg_len, at::IntArrayR
   }
 }
 
+// Document intervals int32 [world, b, n, 2] (parallel/documents.py), or null: document masking off.
+const int* doc_spans_ptr(const c10::optional<Tensor>& spans, int world, int batch, int n_q, int n_k,
+                         int64_t q_pos_offset) {
+  if (!spans.has_value()) return nullptr;
+  const Tensor& t = *spans;
+  TORCH_CHECK(n_q == n_k && q_pos_offset == 0, "document masking needs self-attention (n_q == n_k)");
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.is_contiguous() && t.dim() == 4 && t.size(0) == world &&
+                  t.size(1) == batch && t.size(2) == n_k && t.size(3) == 2,
+              "doc_spans must be contiguous int32 [world, b, n, 2]");
+  return t.data_ptr<int>();
+}
+
 // Hop mode (memory = "ring"): kv_buf holds ONE owner's slot ([1, 2, b*hk, n_k, d]); the launch visits that owner only
 // and carries the online-softmax state (un-normalised O, running max / sum) in fp32 buffers between launches.
 struct FwdHop {
@@ -73,7 +85,7 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
                                          bool causal, int64_t window, double scale, double softclamp,
                                          int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                          at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
-                                         const FwdHop& hop) {
+                                         const FwdHop& hop, const c10::optional<Tensor>& doc_spans) {
   check_16bit(q, "q");
   check_16bit(kv_buf, "kv_buf");
   const bool hop_mode = hop.owner >= 0;
@@ -119,6 +131,7 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
     p.kmask_bits = reinterpret_cast<const uint32_t*>(km.data_ptr<int>());
     p.kmask_words = km.size(2);
   }
+  p.doc_spans = doc_spans_ptr(doc_spans, world, b, n_q, n_k, q_pos_offset);
   p.slot_bytes = 2ull * b * kv_heads * n_k * d * 2;
   // the kernels address owner o's K / V at slot o of the buffer; in hop mode the one slot we were given IS slot
   // `owner`, so the base is shifted down by owner slots (only that slot is ever dereferenced)
@@ -161,9 +174,10 @@ std::tuple<Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& kv_buf, at::I
                                     const Tensor& ready, const c10::optional<Tensor>& kmask_bits,
                                     int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
                                     double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
-                                    at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner) {
+                                    at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
+                                    const c10::optional<Tensor>& doc_spans) {
   return attn_fwd_impl(q, kv_buf, peer_ptrs, ready, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
-                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{});
+                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{}, doc_spans);
 }
 
 // One ring hop of the forward: q against owner `owner`'s K / V slot.  carry_o fp32 [b, n_q, h, d] and carry_ml fp32
@@ -173,7 +187,8 @@ std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, 
                                         const c10::optional<Tensor>& kmask_bits, int64_t kv_heads, int64_t rank,
                                         bool causal, int64_t window, double scale, double softclamp,
                                         int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
-                                        at::IntArrayRef base1, int64_t q_pos_offset) {
+                                        at::IntArrayRef base1, int64_t q_pos_offset,
+                                        const c10::optional<Tensor>& doc_spans) {
   TORCH_CHECK(q.dim() == 4);
   const int64_t b = q.size(0), n_q = q.size(1), h = q.size(2), d = q.size(3);
   TORCH_CHECK(carry_o.is_cuda() && carry_o.scalar_type() == at::kFloat && carry_o.is_contiguous() &&
@@ -190,7 +205,7 @@ std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, 
   hop.carry_out = carry_out;
   const int64_t owners[1] = {owner};
   return attn_fwd_impl(q, kv_slot, {}, c10::nullopt, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
-                       pos_stride, seg_len, base0, base1, q_pos_offset, at::IntArrayRef(owners, 1), hop);
+                       pos_stride, seg_len, base0, base1, q_pos_offset, at::IntArrayRef(owners, 1), hop, doc_spans);
 }
 
 
@@ -225,7 +240,7 @@ BwdSetup make_bwd_setup(const Tensor& qdo_buf, const Tensor& kv_buf, const Tenso
                         const c10::optional<Tensor>& kmask_bits, int64_t batch, int64_t heads, int64_t kv_heads,
                         int64_t rank, bool causal, int64_t window, double scale, double softclamp, int64_t pos_stride,
                         int64_t seg_len, at::IntArrayRef base0, at::IntArrayRef base1, int64_t q_pos_offset,
-                        at::IntArrayRef hop_owner) {
+                        at::IntArrayRef hop_owner, const c10::optional<Tensor>& doc_spans) {
   check_16bit(qdo_buf, "qdo_buf");
   check_16bit(kv_buf, "kv_buf");
   TORCH_CHECK(qdo_buf.is_contiguous() && kv_buf.is_contiguous() && stat_buf.is_contiguous());
@@ -262,6 +277,7 @@ BwdSetup make_bwd_setup(const Tensor& qdo_buf, const Tensor& kv_buf, const Tenso
     p.ready = reinterpret_cast<const uint32_t*>(ready->data_ptr<int>());
     p.ready_target = (uint32_t)ready_target;
   }
+  p.doc_spans = doc_spans_ptr(doc_spans, world, (int)batch, n_q, n_k, q_pos_offset);
   uint64_t qdims[4] = {(uint64_t)d, (uint64_t)n_q, (uint64_t)batch * heads, (uint64_t)2 * world};
   uint64_t qstr[3] = {(uint64_t)d * 2, (uint64_t)n_q * d * 2, (uint64_t)batch * heads * n_q * d * 2};
   uint32_t qbox128[4] = {64, 128, 1, 1};
@@ -279,11 +295,12 @@ Tensor attn_bwd_dq(const Tensor& qdo_buf, const Tensor& kv_buf, const Tensor& st
                    const c10::optional<Tensor>& ready, int64_t ready_target, const c10::optional<Tensor>& kmask_bits,
                    int64_t batch, int64_t heads, int64_t kv_heads, int64_t rank, bool causal, int64_t window,
                    double scale, double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
-                   at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner) {
+                   at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
+                   const c10::optional<Tensor>& doc_spans) {
   c10::cuda::CUDAGuard guard(kv_buf.device());
   BwdSetup s = make_bwd_setup(qdo_buf, kv_buf, stat_buf, ready, ready_target, kmask_bits, batch, heads, kv_heads, rank,
                               causal, window, scale, softclamp, pos_stride, seg_len, base0, base1, q_pos_offset,
-                              hop_owner);
+                              hop_owner, doc_spans);
   const int d = kv_buf.size(4);
   Tensor dq = torch::empty({batch, s.p.n_q, heads, d}, kv_buf.options());
   s.p.dq = dq.data_ptr();
@@ -301,11 +318,12 @@ std::tuple<Tensor, Tensor> attn_bwd_dkdv(const Tensor& qdo_buf, const Tensor& kv
                                          const c10::optional<Tensor>& kmask_bits, int64_t batch, int64_t heads,
                                          int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
                                          double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
-                                         at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner) {
+                                         at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
+                                         const c10::optional<Tensor>& doc_spans) {
   c10::cuda::CUDAGuard guard(kv_buf.device());
   BwdSetup s = make_bwd_setup(qdo_buf, kv_buf, stat_buf, ready, ready_target, kmask_bits, batch, heads, kv_heads, rank,
                               causal, window, scale, softclamp, pos_stride, seg_len, base0, base1, q_pos_offset,
-                              hop_owner);
+                              hop_owner, doc_spans);
   const int d = kv_buf.size(4);
   Tensor dk = torch::empty({batch, s.p.n_k, kv_heads, d}, kv_buf.options());
   Tensor dv = torch::empty({batch, s.p.n_k, kv_heads, d}, kv_buf.options());
@@ -334,7 +352,7 @@ std::tuple<Tensor, Tensor> attn_bwd_ring(const Tensor& qdo, const Tensor& kv_buf
                                          double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                          at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
                                          at::IntArrayRef dkv_acc_ptrs, int64_t nk_pad, int64_t world_size,
-                                         int64_t slot_owner) {
+                                         int64_t slot_owner, const c10::optional<Tensor>& doc_spans) {
   // slot_owner >= 0 (memory = "ring"): kv_buf is ONE owner's slot [1, 2, b*hk, n_k, d] of a `world_size` ring and
   // hop_owner == [slot_owner]; dq_acc and the dK / dV accumulators keep adding up across the per-hop launches
   check_16bit(qdo, "qdo");
@@ -386,6 +404,7 @@ std::tuple<Tensor, Tensor> attn_bwd_ring(const Tensor& qdo, const Tensor& kv_buf
     p.ready = reinterpret_cast<const uint32_t*>(ready->data_ptr<int>());
     p.ready_target = (uint32_t)ready_target;
   }
+  p.doc_spans = doc_spans_ptr(doc_spans, world, (int)batch, n_q, n_k, q_pos_offset);
   // local Q / dO: dims (d, n_q, b*h, 2), box (64, 64, 1, 1)
   uint64_t qdims[4] = {(uint64_t)d, (uint64_t)n_q, (uint64_t)batch * heads, 2};
   uint64_t qstr[3] = {(uint64_t)d * 2, (uint64_t)n_q * d * 2, (uint64_t)batch * heads * n_q * d * 2};
@@ -634,7 +653,7 @@ void symm_close(int64_t ptr) { rab::symm_close(reinterpret_cast<void*>(ptr)); }
 TORCH_LIBRARY(rab, m) {
   m.def("attn_fwd(Tensor q, Tensor kv_buf, int[] peer_ptrs, Tensor ready, Tensor? kmask_bits, int kv_heads, int rank, "
         "bool causal, int window, float scale, float softclamp, int pos_stride, int seg_len, int[] base0, int[] "
-        "base1, int q_pos_offset, int[] hop_owner) -> (Tensor, Tensor)");
+        "base1, int q_pos_offset, int[] hop_owner, Tensor? doc_spans=None) -> (Tensor, Tensor)");
   m.def("pack_kv(Tensor k, Tensor v, Tensor(a!) slot, int which=3) -> ()");
   m.def("rotary(Tensor x, Tensor angles, Tensor(a!) out, bool head_major, float sign) -> ()");
   m.def("tree_decode(Tensor q, Tensor? k, Tensor? v, Tensor? k_scale, Tensor? v_scale, Tensor(a!) scratch, Tensor(b!) "
@@ -645,18 +664,20 @@ TORCH_LIBRARY(rab, m) {
   m.def("bwd_prep(Tensor q, Tensor o, Tensor dout, Tensor lse, Tensor(a!) qdo_buf, Tensor(b!) stat_buf, int rank) -> ()");
   m.def("attn_bwd_dq(Tensor qdo_buf, Tensor kv_buf, Tensor stat_buf, Tensor? ready, int ready_target, Tensor? "
         "kmask_bits, int batch, int heads, int kv_heads, int rank, bool causal, int window, float scale, float "
-        "softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner) -> Tensor");
+        "softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner, Tensor? "
+        "doc_spans=None) -> Tensor");
   m.def("attn_bwd_dkdv(Tensor qdo_buf, Tensor kv_buf, Tensor stat_buf, Tensor? ready, int ready_target, Tensor? "
         "kmask_bits, int batch, int heads, int kv_heads, int rank, bool causal, int window, float scale, float "
-        "softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner) -> "
-        "(Tensor, Tensor)");
+        "softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner, Tensor? "
+        "doc_spans=None) -> (Tensor, Tensor)");
   m.def("attn_bwd_ring(Tensor qdo, Tensor kv_buf, Tensor stat, Tensor(a!) dq_acc, Tensor? ready, int ready_target, "
         "Tensor? kmask_bits, int batch, int heads, int kv_heads, int rank, bool causal, int window, float scale, float "
         "softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner, int[] "
-        "dkv_acc_ptrs, int nk_pad, int world_size=0, int slot_owner=-1) -> (Tensor, Tensor)");
+        "dkv_acc_ptrs, int nk_pad, int world_size=0, int slot_owner=-1, Tensor? doc_spans=None) -> (Tensor, Tensor)");
   m.def("attn_fwd_hop(Tensor q, Tensor kv_slot, int owner, int world, Tensor(a!) carry_o, Tensor(b!) carry_ml, bool "
         "carry_in, bool carry_out, Tensor? kmask_bits, int kv_heads, int rank, bool causal, int window, float scale, "
-        "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset) -> (Tensor, Tensor)");
+        "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None) "
+        "-> (Tensor, Tensor)");
   m.def("acc_convert(Tensor acc, Tensor(a!) out, float scale) -> ()");
   m.def("set_fetch_timing(Tensor? times) -> ()");
   m.def("device_barrier(int[] pad_ptrs, int rank, int epoch) -> ()");

@@ -62,6 +62,8 @@ struct AttnFwdParams {
   int carry_in;      // 1: initialise O / m / l of every item from the carry buffers
   int carry_out;     // 1: store the un-normalised state instead of the final O / lse
   int all_ready;     // 1: every slot this launch reads is already complete (no in-kernel fetch, no ready flags)
+  // document spans int32 [world][batch][n][2]: [start, end) global positions of each token's document (null = off)
+  const int* doc_spans;
 };
 
 template <int D>
@@ -96,6 +98,7 @@ struct AttnBwdParams {
   int kmask_words;
   const uint32_t* ready;       // [world] flags: slot o usable once ready[o] >= ready_target (may be null)
   uint32_t ready_target;
+  const int* doc_spans;        // [world][batch][n][2] document intervals, null = off (see AttnFwdParams)
 };
 
 template <int D>
@@ -133,6 +136,7 @@ struct AttnBwdFusedParams {
   float* dq_acc;
   int ring_reduce;
   float* dkv_acc[kMaxWorld];
+  const int* doc_spans;      // [world][batch][n][2] document intervals, null = off (see AttnFwdParams)
 };
 void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdFusedParams& p,
                            int num_sms, cudaStream_t stream);

@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from torch import Tensor, nn
 from torch.nn import Module, ModuleList
 
-from ring_attention_pytorch_b200.ops.oracle import default_attention
+from ring_attention_pytorch_b200.ops.oracle import attention_with_positions, default_attention
 from ring_attention_pytorch_b200.ops.ring_flash_naive import ring_flash_attn
 from ring_attention_pytorch_b200.parallel.distributed import (
     AllGather,
@@ -36,6 +36,7 @@ from ring_attention_pytorch_b200.parallel.distributed import (
     is_distributed,
     split_by_rank,
 )
+from ring_attention_pytorch_b200.parallel.documents import document_runs
 from ring_attention_pytorch_b200.parallel.layout import make_position_map
 from ring_attention_pytorch_b200.utils.validate import typecheck
 
@@ -121,6 +122,15 @@ def maybe_pad_seq_and_mask(x: Tensor, mask: Optional[Tensor], seq_size: int):
     if mask is None:
         mask = torch.ones(x.shape[:2], device=x.device, dtype=torch.bool)
     return _pad_tokens(x, seq_size, 0), _pad_tokens(mask, seq_size, False)
+
+
+def pad_document_ids(document_ids: Tensor, seq_size: int) -> Tensor:
+    """Right-pad ``[b, n]`` document ids to a multiple of ``seq_size`` with an id that differs from each row's last one,
+    so the padding is a document of its own."""
+    missing = -document_ids.shape[1] % seq_size
+    if missing == 0:
+        return document_ids
+    return torch.cat((document_ids, (document_ids[:, -1:] + 1).expand(-1, missing)), dim=1)
 
 
 def stripe(t: Tensor, ring_seq_size: int) -> Tensor:
@@ -296,7 +306,11 @@ class RingAttention(Module):
         rotary_emb: Optional[Tensor] = None,
         force_ring_reduce_off: bool = False,
         ring_size: Optional[int] = None,
+        document_ids: Optional[Tensor] = None,
     ) -> Tensor:
+        """``document_ids`` (integer ``[b, n]``, laid out like ``x``): document masking for packed sequences, see
+        :func:`ring_attention_pytorch_b200.ops.ring_cuda.ring_flash_attn_cuda`.  It follows ``x`` through the padding,
+        striping and sharding, and is honoured by every attention path."""
         ring_size = default(ring_size, get_world_size())
         ring_attn = self.ring_attn and is_distributed()
         auto_shard_seq = self.auto_shard_seq and is_distributed()
@@ -304,11 +318,17 @@ class RingAttention(Module):
 
         if auto_shard_seq:
             x, mask = maybe_pad_seq_and_mask(x, mask, self.ring_seq_size)
+            if exists(document_ids):
+                document_ids = pad_document_ids(document_ids, self.ring_seq_size)
             if self.striped_ring_attn:
                 x = stripe(x, self.ring_seq_size)
                 if exists(mask):
                     mask = stripe(mask, self.ring_seq_size)
+                if exists(document_ids):
+                    document_ids = stripe(document_ids, self.ring_seq_size)
             (x, mask), batch_sizes, num_sharded_batches = sharded_batch_to_sharded_seq(x, mask, self.ring_seq_size)
+            if exists(document_ids):
+                (document_ids, _), *_ = sharded_batch_to_sharded_seq(document_ids, None, self.ring_seq_size)
             ring_size = get_world_size() // num_sharded_batches
 
         qkv = self.to_qkv(x)
@@ -328,17 +348,22 @@ class RingAttention(Module):
             q = apply_rotary_pos_emb(rotary_emb, q)
             k = apply_rotary_pos_emb(rotary_emb, k)
 
-        if self.force_regular_attn:
+        if self.force_regular_attn and exists(document_ids):
+            runs = document_runs(document_ids)
+            out = attention_with_positions(q, k, v, causal=self.causal, key_mask=None if self.causal else mask,
+                                           q_doc=runs, k_doc=runs)
+        elif self.force_regular_attn:
             out = default_attention(q, k, v, mask=mask, causal=self.causal)
         elif kernel_path:
             from ring_attention_pytorch_b200.ops.ring_cuda import ring_flash_attn_cuda
 
             out = ring_flash_attn_cuda(q, k, v, mask, self.causal, self.bucket_size, use_ring,
                                        self.striped_ring_attn and use_ring, self.max_lookback_seq_len, ring_size,
-                                       rotary_freqs=rotary_emb if fuse_rotary else None)
+                                       rotary_freqs=rotary_emb if fuse_rotary else None, document_ids=document_ids)
         else:
             out = ring_flash_attn(q, k, v, mask, self.causal, self.bucket_size, use_ring,
-                                  self.striped_ring_attn and use_ring, self.max_lookback_seq_len, ring_size)
+                                  self.striped_ring_attn and use_ring, self.max_lookback_seq_len, ring_size,
+                                  document_ids=document_ids)
 
         out = out.reshape(b, n, -1)
         out = self.to_out(out)
@@ -421,7 +446,10 @@ class RingTransformer(Module):
         return_loss: bool = False,
         force_ring_reduce_off: bool = False,
         ring_size: Optional[int] = None,
+        document_ids: Optional[Tensor] = None,
     ):
+        """``document_ids`` (integer ``[b, n]``, like ``x``): packed-sequence document masking in every layer (see
+        :class:`RingAttention`); with ``return_loss`` it is shifted together with the input."""
         seq_len = x.shape[-1]
         auto_shard_seq = not force_ring_reduce_off and self.auto_shard_seq and is_distributed()
         use_ring = self.ring_attn and is_distributed() and not force_ring_reduce_off
@@ -432,6 +460,8 @@ class RingTransformer(Module):
             # label i is token i + 1: its validity is the mask of token i + 1 (reference ring_attention.py:614 uses
             # mask[:, 1:] as well); the input mask loses its last position together with the input
             x, labels = x[:, :-1], x[:, 1:]
+            if exists(document_ids):
+                document_ids = document_ids[:, :-1]
             if exists(mask):
                 label_mask = mask[:, 1:]
                 mask = mask[:, :-1]
@@ -442,6 +472,8 @@ class RingTransformer(Module):
 
         if auto_shard_seq:
             x, mask = maybe_pad_seq_and_mask(x, mask, self.ring_seq_size)
+            if exists(document_ids):
+                document_ids = pad_document_ids(document_ids, self.ring_seq_size)
             if exists(labels):
                 labels, label_mask = maybe_pad_seq_and_mask(labels, label_mask, self.ring_seq_size)
                 if exists(label_mask):
@@ -453,9 +485,13 @@ class RingTransformer(Module):
                     labels = stripe(labels, self.ring_seq_size)
                 if exists(mask):
                     mask = stripe(mask, self.ring_seq_size)
+                if exists(document_ids):
+                    document_ids = stripe(document_ids, self.ring_seq_size)
             (x, mask), batch_sizes, num_sharded_batches = sharded_batch_to_sharded_seq(x, mask, self.ring_seq_size)
             if exists(labels):
                 (labels, _), *_ = sharded_batch_to_sharded_seq(labels, None, self.ring_seq_size)
+            if exists(document_ids):
+                (document_ids, _), *_ = sharded_batch_to_sharded_seq(document_ids, None, self.ring_seq_size)
             ring_size = get_world_size() // num_sharded_batches
 
         if exists(labels) and exists(label_mask):  # not auto-sharded: padded targets are ignored as well
@@ -470,7 +506,7 @@ class RingTransformer(Module):
         x = self.token_emb(x)
         for attn, ff in self.layers:
             x = attn(x, mask=mask, rotary_emb=rotary_emb, force_ring_reduce_off=force_ring_reduce_off,
-                     ring_size=ring_size) + x
+                     ring_size=ring_size, document_ids=document_ids) + x
             x = ff(x) + x
         logits = self.to_logits(x)
 

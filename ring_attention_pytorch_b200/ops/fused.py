@@ -5,6 +5,9 @@ compose; they are also what the GPU unit tests drive directly.  ``emulate_ring_f
 W-rank ring on ONE device by giving every emulated rank its own K/V gather buffer and pointing the
 "peer" addresses at the other ranks' buffers – the kernel cannot tell the difference, which lets the
 multi-hop fetch/ready-flag protocol be tested on a single GPU.
+
+``doc_spans`` (every wrapper) is the int32 ``[world, b, n, 2]`` document interval table of
+:mod:`ring_attention_pytorch_b200.parallel.documents`; ``None`` launches the kernels without document masking.
 """
 from __future__ import annotations
 
@@ -13,6 +16,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from ring_attention_pytorch_b200.ops import _ext
+from ring_attention_pytorch_b200.parallel.documents import document_spans
 from ring_attention_pytorch_b200.parallel.layout import (PositionMap, make_position_map, ring_hop_owners,
                                                           ring_query_owners)
 
@@ -50,12 +54,13 @@ def fused_attn_fwd(
     softclamp: float = 0.0,
     q_pos_offset: int = 0,
     hop_owner: Optional[List[int]] = None,
+    doc_spans: Optional[torch.Tensor] = None,
 ):
     if hop_owner is None:
         hop_owner = ring_hop_owners(pm, rank, causal, window)
     return _ext.ops().attn_fwd(
         q, kv_buf, list(peer_ptrs), ready, kmask_bits, kv_heads, rank, bool(causal), int(window or 0), float(scale),
-        float(softclamp), pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), list(hop_owner))
+        float(softclamp), pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), list(hop_owner), doc_spans)
 
 
 def fused_attn_fwd_hop(
@@ -77,6 +82,7 @@ def fused_attn_fwd_hop(
     scale: float,
     softclamp: float = 0.0,
     q_pos_offset: int = 0,
+    doc_spans: Optional[torch.Tensor] = None,
 ):
     """ONE ring hop of the forward (``memory="ring"``): ``q`` against owner ``owner``'s K/V slot ``[2, b*hk, n_k, d]``.
 
@@ -87,7 +93,7 @@ def fused_attn_fwd_hop(
     return _ext.ops().attn_fwd_hop(
         q, kv_slot[None], int(owner), int(world), carry_o, carry_ml, bool(carry_in), bool(carry_out), kmask_bits,
         kv_heads, rank, bool(causal), int(window or 0), float(scale), float(softclamp), pm.stride, pm.seg_len, pm.base0,
-        pm.base1, int(q_pos_offset))
+        pm.base1, int(q_pos_offset), doc_spans)
 
 
 def alloc_fwd_carry(q: torch.Tensor):
@@ -108,11 +114,13 @@ def emulate_ring_forward(
     key_masks: Optional[Sequence[torch.Tensor]] = None,
     scale: Optional[float] = None,
     hopwise: bool = False,
+    document_ids: Optional[Sequence[torch.Tensor]] = None,
 ):
     """Run the fused forward for every rank of a W-rank ring on the current device.
 
     qs/ks/vs: per-rank shards ``[b, n, h, d]`` / ``[b, n, hk, d]``.  Returns (outs, lses) lists.
     ``hopwise``: one launch per hop with carried softmax state (the ``memory="ring"`` schedule).
+    ``document_ids``: per-rank ``[b, n]`` document ids (in the ring's layout) for document masking.
     """
     ops = _ext.ops()
     world = len(qs)
@@ -128,6 +136,7 @@ def emulate_ring_forward(
     kbits = None
     if key_masks is not None:
         kbits = pack_key_mask_bits(torch.stack(list(key_masks), 0))
+    spans = None if document_ids is None else document_spans(torch.stack(list(document_ids), 0), pm)
     outs, lses = [], []
     if hopwise:
         for r in range(world):
@@ -137,7 +146,8 @@ def emulate_ring_forward(
             for s_, owner in enumerate(hops):
                 o, lse = fused_attn_fwd_hop(q, bufs[owner][owner], owner, world, carry_o, carry_ml, kbits,
                                             carry_in=s_ > 0, carry_out=s_ + 1 < len(hops), kv_heads=hk, rank=r, pm=pm,
-                                            causal=causal, window=window, scale=scale, softclamp=softclamp)
+                                            causal=causal, window=window, scale=scale, softclamp=softclamp,
+                                            doc_spans=spans)
             outs.append(o)
             lses.append(lse)
         return outs, lses
@@ -145,7 +155,7 @@ def emulate_ring_forward(
         ready = torch.zeros(world, dtype=torch.int32, device=dev)
         peers = [bufs[o][o].data_ptr() for o in range(world)]  # owner o's own slot
         o, lse = fused_attn_fwd(qs[r].contiguous(), bufs[r], peers, ready, kbits, kv_heads=hk, rank=r, pm=pm,
-                                causal=causal, window=window, scale=scale, softclamp=softclamp)
+                                causal=causal, window=window, scale=scale, softclamp=softclamp, doc_spans=spans)
         outs.append(o)
         lses.append(lse)
     return outs, lses
@@ -182,6 +192,7 @@ def fused_attn_bwd(
     ready_kv: Optional[torch.Tensor] = None,
     ready_q: Optional[torch.Tensor] = None,
     ready_target: int = 0,
+    doc_spans: Optional[torch.Tensor] = None,
 ):
     """Run both backward kernels on already gathered buffers; returns (dq, dk, dv)."""
     ops = _ext.ops()
@@ -189,8 +200,8 @@ def fused_attn_bwd(
     q_owners = ring_query_owners(pm, rank, causal, window)
     common = (kmask_bits, batch, heads, kv_heads, rank, bool(causal), int(window or 0), float(scale), float(softclamp),
               pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset))
-    dq = ops.attn_bwd_dq(qdo_buf, kv_buf, stat_buf, ready_kv, ready_target, *common, kv_owners)
-    dk, dv = ops.attn_bwd_dkdv(qdo_buf, kv_buf, stat_buf, ready_q, ready_target, *common, q_owners)
+    dq = ops.attn_bwd_dq(qdo_buf, kv_buf, stat_buf, ready_kv, ready_target, *common, kv_owners, doc_spans)
+    dk, dv = ops.attn_bwd_dkdv(qdo_buf, kv_buf, stat_buf, ready_q, ready_target, *common, q_owners, doc_spans)
     return dq, dk, dv
 
 
@@ -222,6 +233,7 @@ def fused_attn_bwd_ring(
     hop_owner: Optional[List[int]] = None,
     world: int = 0,
     slot_owner: int = -1,
+    doc_spans: Optional[torch.Tensor] = None,
 ):
     """The one-kernel (5-GEMM) backward, head dim 128 (``csrc/attn_bwd_sm90.cu``, KV-stationary kernel in its one-pass form).
 
@@ -242,7 +254,7 @@ def fused_attn_bwd_ring(
     dk, dv = ops.attn_bwd_ring(qdo, kv_buf, stat, dq_acc, ready, int(ready_target), kmask_bits, batch, heads, kv_heads,
                                rank, bool(causal), int(window or 0), float(scale), float(softclamp), pm.stride,
                                pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), list(hop_owner),
-                               list(dkv_acc_ptrs), int(nk_pad), int(world), int(slot_owner))
+                               list(dkv_acc_ptrs), int(nk_pad), int(world), int(slot_owner), doc_spans)
     return dq_acc, dk, dv
 
 
@@ -256,6 +268,7 @@ def emulate_ring_backward(
     scale: Optional[float] = None,
     fused: Optional[bool] = None,
     hopwise: bool = False,
+    document_ids=None,
 ):
     """Backward of :func:`emulate_ring_forward` for every emulated rank on the current device.
     ``hopwise`` (fused only): one launch per hop against a single K/V slot (the ``memory="ring"`` schedule).
@@ -279,6 +292,7 @@ def emulate_ring_backward(
     kbits = None
     if key_masks is not None:
         kbits = pack_key_mask_bits(torch.stack(list(key_masks), 0))
+    spans = None if document_ids is None else document_spans(torch.stack(list(document_ids), 0), pm)
     if fused is None:
         fused = d == 128
     res = []
@@ -295,11 +309,13 @@ def emulate_ring_backward(
                     dq_acc, dk, dv = fused_attn_bwd_ring(
                         qdo_all[r], stat_all[r], kv_all[owner:owner + 1], kbits, batch=b, heads=h, kv_heads=hk, rank=r,
                         pm=pm, causal=causal, window=window, scale=scale, softclamp=softclamp, dq_acc=dq_acc,
-                        dkv_acc_ptrs=ptrs, nk_pad=nk_pad, hop_owner=[owner], world=world, slot_owner=owner)
+                        dkv_acc_ptrs=ptrs, nk_pad=nk_pad, hop_owner=[owner], world=world, slot_owner=owner,
+                        doc_spans=spans)
             else:
                 dq_acc, dk, dv = fused_attn_bwd_ring(qdo_all[r], stat_all[r], kv_all, kbits, batch=b, heads=h,
                                                      kv_heads=hk, rank=r, pm=pm, causal=causal, window=window,
-                                                     scale=scale, softclamp=softclamp, dkv_acc_ptrs=ptrs, nk_pad=nk_pad)
+                                                     scale=scale, softclamp=softclamp, dkv_acc_ptrs=ptrs, nk_pad=nk_pad,
+                                                     doc_spans=spans)
             dqs.append(dq_acc)
             direct.append((dk, dv))
         for r in range(world):
@@ -317,5 +333,5 @@ def emulate_ring_backward(
     for r in range(world):
         # every emulated rank sees the same fully gathered buffers (what the NVLink gather produces)
         res.append(fused_attn_bwd(qdo_all, kv_all, stat_all, kbits, batch=b, heads=h, kv_heads=hk, rank=r, pm=pm,
-                                  causal=causal, window=window, scale=scale, softclamp=softclamp))
+                                  causal=causal, window=window, scale=scale, softclamp=softclamp, doc_spans=spans))
     return res

@@ -45,9 +45,13 @@ def attention_with_positions(
     softclamp_value: float = 0.0,
     scale: Optional[float] = None,
     return_lse: bool = False,
+    q_doc: Optional[Tensor] = None,
+    k_doc: Optional[Tensor] = None,
 ):
     """q [b, i, h, d]; k, v [b, j, hk, d]; q_pos [i], k_pos [j] integer global positions.
 
+    ``q_doc`` [b, i] / ``k_doc`` [b, j]: document labels, a query sees only keys with its label (on top of every other
+    rule).  Labels must be unique per document, e.g. the start column of ``parallel.documents.document_spans``.
     Rows with no visible key produce zeros (and ``lse = +inf``).
     """
     b, i, h, d = q.shape
@@ -70,6 +74,8 @@ def attention_with_positions(
         visible = visible & vis[None, None]
     if key_mask is not None:
         visible = visible & key_mask[:, None, None, :]
+    if q_doc is not None:
+        visible = visible & (q_doc[:, None, :, None] == k_doc[:, None, None, :])
     neg = torch.finfo(sim.dtype).min
     sim = sim.masked_fill(~visible, neg)
     any_vis = visible.any(dim=-1, keepdim=True)

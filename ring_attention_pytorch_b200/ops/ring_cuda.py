@@ -60,6 +60,7 @@ from ring_attention_pytorch_b200.ops.fused import (
     pad128,
 )
 from ring_attention_pytorch_b200.parallel.distributed import default, exists, get_rank, get_world_size, is_distributed
+from ring_attention_pytorch_b200.parallel.documents import check_document_ids, ring_document_spans
 from ring_attention_pytorch_b200.parallel.layout import make_position_map, ring_hop_owners, ring_query_owners
 from ring_attention_pytorch_b200.parallel.symm import get_workspace
 from ring_attention_pytorch_b200.utils.timing import nvtx_range
@@ -195,6 +196,7 @@ class RingFlashAttentionCUDAFunction(Function):
         softclamp_value: float = 50.0,
         layout: Optional[str] = None,
         rotary_freqs: Optional[Tensor] = None,
+        document_ids: Optional[Tensor] = None,
     ):
         assert q.is_cuda and k.is_cuda and v.is_cuda, "ring_flash_attn_cuda needs CUDA tensors"
         ops = _ext.ops()
@@ -247,6 +249,8 @@ class RingFlashAttentionCUDAFunction(Function):
         pm = make_position_map(layout, ring_size, n_k)
         q_off = (n_k - n_q) if (cross_attn and causal) else 0
         dev = q.device
+        # document masking: the [ring, b, n, 2] interval table, built once here and reused by every launch of the backward
+        spans = ring_document_spans(document_ids.to(dev), pm, use_ring) if exists(document_ids) else None
 
         ready = torch.zeros(ring_size, dtype=torch.int32, device=dev)
         peers = [0] * ring_size
@@ -288,14 +292,14 @@ class RingFlashAttentionCUDAFunction(Function):
                     o, lse = fused_attn_fwd_hop(qp, window_slots.slot(s_), owner, ring_size, carry_o, carry_ml, kbits,
                                                 carry_in=s_ > 0, carry_out=s_ + 1 < len(hops), kv_heads=hk, rank=rank,
                                                 pm=pm, causal=causal, window=max_lookback_seq_len, scale=scale,
-                                                softclamp=softclamp, q_pos_offset=q_off)
+                                                softclamp=softclamp, q_pos_offset=q_off, doc_spans=spans)
                     window_slots.launched(s_)
                     _count()
                 del carry_o, carry_ml
             else:
                 o, lse = fused_attn_fwd(qp, kv_gather, peers, ready, kbits, kv_heads=hk, rank=rank, pm=pm,
                                         causal=causal, window=max_lookback_seq_len, scale=scale, softclamp=softclamp,
-                                        q_pos_offset=q_off)
+                                        q_pos_offset=q_off, doc_spans=spans)
                 _count()
 
         ctx.cfg = (causal, max_lookback_seq_len, ring_size, rank, layout, softclamp, scale, q_off, use_ring, d, d_pad,
@@ -304,7 +308,7 @@ class RingFlashAttentionCUDAFunction(Function):
         none = torch.empty(0, device=dev)
         ctx.save_for_backward(qp, kp if use_ring else none, vp if use_ring else none, o, lse,
                               none if use_ring else kv_gather, kbits if kbits is not None else none,
-                              ang if ang is not None else none)
+                              ang if ang is not None else none, spans if spans is not None else none)
         out = o[..., :d]
         return out.to(orig_dtype) if orig_dtype != dt else out
 
@@ -313,9 +317,10 @@ class RingFlashAttentionCUDAFunction(Function):
         ops = _ext.ops()
         (causal, window, ring_size, rank, layout, softclamp, scale, q_off, use_ring, d, d_pad, orig_dtype,
          hk, fused_k_rotary) = ctx.cfg
-        qp, kp, vp, o, lse, kv_saved, kbits, ang = ctx.saved_tensors
+        qp, kp, vp, o, lse, kv_saved, kbits, ang, spans = ctx.saved_tensors
         kbits = kbits if kbits.numel() > 0 else None
         ang = ang if ang.numel() > 0 else None
+        spans = spans if spans.numel() > 0 else None
         dt = qp.dtype
         b, n_q, h, _ = qp.shape
         dev = qp.device
@@ -389,7 +394,7 @@ class RingFlashAttentionCUDAFunction(Function):
                                             kv_heads=hk, rank=rank, pm=pm, causal=causal, window=window, scale=scale,
                                             softclamp=softclamp, q_pos_offset=q_off, dq_acc=dq_acc,
                                             dkv_acc_ptrs=acc_ptrs, nk_pad=nk_pad, hop_owner=[owner], world=ring_size,
-                                            slot_owner=owner)
+                                            slot_owner=owner, doc_spans=spans)
                         window_slots.launched(s_)
                         _count()
                     _count(-1)
@@ -398,7 +403,7 @@ class RingFlashAttentionCUDAFunction(Function):
                                                     rank=rank, pm=pm, causal=causal, window=window, scale=scale,
                                                     softclamp=softclamp, q_pos_offset=q_off, dq_acc=dq_acc,
                                                     dkv_acc_ptrs=acc_ptrs, nk_pad=nk_pad, ready=ready,
-                                                    ready_target=ready_target, hop_owner=hop_owner)
+                                                    ready_target=ready_target, hop_owner=hop_owner, doc_spans=spans)
                 dq = torch.empty(b, n_q, h, d_pad, dtype=dt, device=dev)
                 ops.acc_convert(dq_acc, dq, scale)
                 _count(2)
@@ -441,11 +446,11 @@ class RingFlashAttentionCUDAFunction(Function):
                       pm.seg_len, pm.base0, pm.base1, int(q_off))
             # dQ only needs the K/V slots (flag per owner): it overlaps with the Q/dO gather
             dq = ops.attn_bwd_dq(qdo_gather, kv_gather, stat_gather, ready_kv, 1 if ready_kv is not None else 0, *common,
-                                 hop_owner)
+                                 hop_owner, spans)
             if gather_done is not None:
                 torch.cuda.current_stream(dev).wait_event(gather_done)
             dk, dv = ops.attn_bwd_dkdv(qdo_gather, kv_gather, stat_gather, None, 0, *common,
-                                       ring_query_owners(pm, rank, causal, window))
+                                       ring_query_owners(pm, rank, causal, window), spans)
             _count(2)
 
         dq, dk, dv = dq[..., :d], dk[..., :d], dv[..., :d]
@@ -457,7 +462,7 @@ class RingFlashAttentionCUDAFunction(Function):
             dq, dk = dq_in, dk_in
         if orig_dtype != dt:
             dq, dk, dv = dq.to(orig_dtype), dk.to(orig_dtype), dv.to(orig_dtype)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 ring_flash_attn_cuda_ = RingFlashAttentionCUDAFunction.apply
@@ -480,12 +485,20 @@ def ring_flash_attn_cuda(
     softclamp_value: float = 50.0,
     layout: Optional[str] = None,
     rotary_freqs: Optional[Tensor] = None,
+    document_ids: Optional[Tensor] = None,
 ) -> Tensor:
     """q [b, n, h, d]; k, v [b, n, hk, d] (this rank's shard when ``ring_reduce_col``).  ``bucket_size`` is
     accepted for signature parity; tiling is fixed by the kernel (128 x 128).  ``rotary_freqs`` ([n, d] or [n, d/2]
     fp32 angles, e.g. the output of ``RingRotaryEmbedding``): rotary embedding of q and k applied inside the op's pack
-    kernels instead of by eager PyTorch passes."""
+    kernels instead of by eager PyTorch passes.
+
+    ``document_ids`` (integer ``[b, n]``, this rank's shard laid out like ``q``): document masking for packed
+    sequences.  A document is a maximal run of equal ids in global position order (two separate runs sharing an id are
+    two documents); a query sees only keys of its own document, on top of ``causal``, the look-back window and
+    ``mask``.  Unlike ``mask`` it is kept under ``causal=True``.  Self-attention only.  Tiles that no document
+    crosses are skipped without being loaded, so packed causal training does only the visible work."""
     check_attention_inputs(q, k, v, mask, name="ring_flash_attn_cuda", max_head_dim=128)
+    check_document_ids(document_ids, q, k)
     return ring_flash_attn_cuda_(q, k, v, mask, causal, bucket_size, ring_reduce_col, striped_ring_attn,
                                  max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value, layout,
-                                 rotary_freqs)
+                                 rotary_freqs, document_ids)

@@ -10,7 +10,8 @@ maps instead of bucket bookkeeping:
 * **correct dK/dV**: the (k, v, dk, dv) packet rides the ring and is sent home once, after the last hop,
   by the exact remaining distance (the reference sends it every iteration and mis-unpacks the result –
   reference ring_flash_attention.py:377-385, SURVEY defect D1/D2/D3);
-* fully masked rows give 0 output (never NaN).
+* fully masked rows give 0 output (never NaN);
+* document masking for packed sequences (``document_ids``, see :mod:`ring_attention_pytorch_b200.parallel.documents`).
 """
 from __future__ import annotations
 
@@ -21,6 +22,7 @@ from torch import Tensor
 from torch.autograd import Function
 
 from ring_attention_pytorch_b200.parallel.distributed import default, exists, get_rank, get_world_size, is_distributed
+from ring_attention_pytorch_b200.parallel.documents import check_document_ids, document_mask, ring_document_spans
 from ring_attention_pytorch_b200.parallel.layout import PositionMap, make_position_map, ring_hop_owners
 from ring_attention_pytorch_b200.parallel.ring import all_ring_pass, null_ring_pass, ring_pass
 from ring_attention_pytorch_b200.utils.validate import check_attention_inputs, typecheck
@@ -77,7 +79,9 @@ class RingFlashAttentionFunction(Function):
         softclamp_qk_sim: bool = False,
         softclamp_value: float = 50.0,
         layout: Optional[str] = None,
+        document_ids: Optional[Tensor] = None,
     ):
+        check_document_ids(document_ids, q, k)
         ring_size = default(ring_size, get_world_size())
         cross_attn = q.shape[-3] != k.shape[-3]
         ring_reduce_col = ring_reduce_col and is_distributed() and not cross_attn and ring_size > 1
@@ -99,6 +103,8 @@ class RingFlashAttentionFunction(Function):
         q_pos = pm.positions(rank, q.device) if not cross_attn else torch.arange(n, device=q.device) + (n_k - n)
         owners = set(ring_hop_owners(pm, rank, causal, max_lookback_seq_len))
         max_iters = ring_num_hops(pm, causal, max_lookback_seq_len) if ring_reduce_col else 1
+        # this rank's query rows: [b, n, 2] intervals of their documents (None: no document masking)
+        q_spans = ring_document_spans(document_ids, pm, ring_reduce_col)[rank] if exists(document_ids) else None
 
         qf = _group_q(q.float() * scale, hk)  # [b, n, g, hk, d]
         o = torch.zeros_like(qf)
@@ -129,6 +135,9 @@ class RingFlashAttentionFunction(Function):
                 if exists(mask_cur):
                     km = mask_cur[:, None, None, None, :]
                     keep = km if keep is None else (keep & km)
+                if exists(q_spans):
+                    dm = document_mask(q_spans[:, s:e], k_pos)[:, :, None, None, :]
+                    keep = dm if keep is None else (keep & dm)
                 if exists(keep):
                     sim = sim.masked_fill(~keep, -torch.finfo(torch.float32).max)
                 blk_max = sim.amax(dim=-1, keepdim=True)
@@ -147,7 +156,7 @@ class RingFlashAttentionFunction(Function):
         out = o.reshape(b, n, h, d).to(q.dtype)
 
         ctx.args = (causal, scale, mask, bucket, ring_reduce_col, ring_size, max_iters, max_lookback_seq_len,
-                    softclamp_qk_sim, softclamp_value, layout, cross_attn, rank)
+                    softclamp_qk_sim, softclamp_value, layout, cross_attn, rank, q_spans)
         ctx.save_for_backward(q, k, v, out, lse)
         return out
 
@@ -155,7 +164,7 @@ class RingFlashAttentionFunction(Function):
     @torch.no_grad()
     def backward(ctx, do: Tensor):
         (causal, scale, mask, bucket, ring_reduce_col, ring_size, max_iters, window, softclamp_qk_sim,
-         softclamp_value, layout, cross_attn, rank) = ctx.args
+         softclamp_value, layout, cross_attn, rank, q_spans) = ctx.args
         q, k, v, o, lse = ctx.saved_tensors
         b, n, h, d = q.shape
         n_k, hk = k.shape[1], k.shape[2]
@@ -198,6 +207,9 @@ class RingFlashAttentionFunction(Function):
                 if exists(mask_cur):
                     km = mask_cur[:, None, None, None, :]
                     keep = km if keep is None else (keep & km)
+                if exists(q_spans):
+                    dm = document_mask(q_spans[:, s:e], k_pos)[:, :, None, None, :]
+                    keep = dm if keep is None else (keep & dm)
                 lse_blk = lse[:, s:e]
                 p = (sim - torch.where(torch.isfinite(lse_blk), lse_blk, torch.zeros_like(lse_blk))).exp()
                 p = torch.where(torch.isfinite(lse_blk), p, torch.zeros_like(p))
@@ -223,7 +235,7 @@ class RingFlashAttentionFunction(Function):
             dk, dv = last_packet[2], last_packet[3]
 
         dq = dq.reshape(b, n, h, d).to(q.dtype)
-        return dq, dk.to(k.dtype), dv.to(v.dtype), None, None, None, None, None, None, None, None, None, None
+        return dq, dk.to(k.dtype), dv.to(v.dtype), None, None, None, None, None, None, None, None, None, None, None
 
 
 ring_flash_attn_ = RingFlashAttentionFunction.apply
@@ -244,8 +256,14 @@ def ring_flash_attn(
     softclamp_qk_sim: bool = False,
     softclamp_value: float = 50.0,
     layout: Optional[str] = None,
+    document_ids: Optional[Tensor] = None,
 ) -> Tensor:
-    """Reference-compatible signature (ring_flash_attention.py:391-406) + ``layout`` ('plain'|'striped'|'zigzag')."""
+    """Reference-compatible signature (ring_flash_attention.py:391-406) + ``layout`` ('plain'|'striped'|'zigzag').
+
+    ``document_ids`` (integer ``[b, n]``, sharded and laid out like ``q``): document masking for packed sequences.  A
+    document is a maximal run of equal ids in global position order (two separate runs sharing an id are two
+    documents); a query sees only keys of its own document, on top of ``causal``, the look-back window and ``mask``.
+    Unlike ``mask`` it is kept under ``causal=True``.  Self-attention only."""
     check_attention_inputs(q, k, v, mask, name="ring_flash_attn")
     return ring_flash_attn_(q, k, v, mask, causal, bucket_size, ring_reduce_col, striped_ring_attn,
-                            max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value, layout)
+                            max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value, layout, document_ids)

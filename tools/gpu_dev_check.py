@@ -22,7 +22,59 @@ sys.path.insert(0, ROOT)
 # ----------------------------------------------------------------------------------------------
 # individual cases (run in a child process: `python tools/gpu_dev_check.py --case NAME`)
 # ----------------------------------------------------------------------------------------------
-def _ref_ring(qs, ks, vs, layout, causal, window, softclamp, key_masks):
+def make_document_ids(kind, b, total, seed=0, device="cuda"):
+    """Global [b, total] document ids of a packed row (``docs=`` option of the cases).
+
+    one    : a single document
+    len1   : documents of length 1 to 4, many of length 1
+    ragged : lengths 1..300, not multiples of the 64 / 128 tiles
+    tiny   : lengths 1..16, many documents inside one tile
+    span   : one document covering everything but 5 tokens at each end (spans every rank of a ring)
+    reuse  : ids alternate between 0 and 1, so separate runs share an id
+    masked : like ragged; with ``kmask`` every key of document 1 is masked (its rows see nothing when non-causal)
+    """
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    if kind == "one":
+        return torch.zeros(b, total, dtype=torch.int64, device=device)
+    if kind == "span":
+        ids = torch.ones(total, dtype=torch.int64)
+        ids[:5], ids[total - 5:] = 0, 2
+        return ids.expand(b, total).contiguous().to(device)
+    if kind == "reuse":
+        return ((torch.arange(total) // 37) % 2).expand(b, total).contiguous().to(device)
+    hi = {"len1": 4, "ragged": 300, "tiny": 16, "masked": 300}[kind]
+    rows = []
+    for _ in range(b):
+        lens = torch.randint(1, hi + 1, (total,), generator=g)
+        if kind == "len1":
+            lens = torch.where(torch.rand(total, generator=g) < 0.5, torch.ones_like(lens), lens)
+        starts = torch.zeros(total, dtype=torch.int64)
+        starts[lens.cumsum(0)[lens.cumsum(0) < total]] = 1
+        rows.append(starts.cumsum(0))
+    return torch.stack(rows).to(device)
+
+
+def _shard_ids(ids, layout, world):
+    from ring_attention_pytorch_b200.parallel.layout import make_position_map
+
+    n = ids.shape[1] // world
+    pm = make_position_map(layout, world, n)
+    return [ids[:, pm.positions(r, ids.device)] for r in range(world)]
+
+
+def _doc_labels(doc_ids, layout, n):
+    """Per-rank document ids -> per-rank run labels for the oracle (start of each token's document)."""
+    import torch
+    from ring_attention_pytorch_b200.parallel.documents import document_spans
+    from ring_attention_pytorch_b200.parallel.layout import make_position_map
+
+    spans = document_spans(torch.stack(doc_ids), make_position_map(layout, len(doc_ids), n))
+    return [spans[r, ..., 0] for r in range(len(doc_ids))]
+
+
+def _ref_ring(qs, ks, vs, layout, causal, window, softclamp, key_masks, doc_ids=None):
     import torch
     from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
     from ring_attention_pytorch_b200.parallel.layout import make_position_map
@@ -34,18 +86,34 @@ def _ref_ring(qs, ks, vs, layout, causal, window, softclamp, key_masks):
     v_all = torch.cat([v.float() for v in vs], 1)
     k_pos = torch.cat([pm.positions(r, qs[0].device) for r in range(world)])
     km = None if key_masks is None else torch.cat(list(key_masks), 1)
+    labels = _doc_labels(doc_ids, layout, n) if doc_ids is not None else None
     outs, lses = [], []
     for r in range(world):
         o, lse = attention_with_positions(qs[r].float(), k_all, v_all, pm.positions(r, qs[0].device), k_pos,
                                           causal=causal, window=window, key_mask=km, softclamp_value=softclamp,
-                                          return_lse=True)
+                                          return_lse=True, q_doc=None if labels is None else labels[r],
+                                          k_doc=None if labels is None else torch.cat(labels, 1))
         outs.append(o)
         lses.append(lse)
     return outs, lses
 
 
+def _case_docs(docs, b, n, world, layout, kmask, seed):
+    """(per-rank document ids, per-rank key masks) of a case."""
+    import torch
+
+    kms = [torch.rand(b, n, device="cuda") > 0.3 for _ in range(world)] if kmask else None
+    if docs is None:
+        return None, kms
+    ids = make_document_ids(docs, b, world * n, seed)
+    doc_ids = _shard_ids(ids, layout, world)
+    if kmask and docs == "masked":
+        kms = [m & (d != 1) for m, d in zip(kms, doc_ids)]
+    return doc_ids, kms
+
+
 def case_fwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=False, window=None, softclamp=0.0,
-             kmask=False, dtype="bf16", seed=0, hopwise=False):
+             kmask=False, dtype="bf16", seed=0, hopwise=False, docs=None):
     import torch
     from ring_attention_pytorch_b200.ops.fused import emulate_ring_forward
 
@@ -55,13 +123,11 @@ def case_fwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=Fa
     qs = [torch.randn(b, n, h, d, device="cuda", dtype=dt) for _ in range(world)]
     ks = [torch.randn(b, n, hk, d, device="cuda", dtype=dt) for _ in range(world)]
     vs = [torch.randn(b, n, hk, d, device="cuda", dtype=dt) for _ in range(world)]
-    kms = None
-    if kmask:
-        kms = [torch.rand(b, n, device="cuda") > 0.3 for _ in range(world)]
+    doc_ids, kms = _case_docs(docs, b, n, world, layout, kmask, seed)
     outs, lses = emulate_ring_forward(qs, ks, vs, layout=layout, causal=causal, window=window, softclamp=softclamp,
-                                      key_masks=kms, hopwise=hopwise)
+                                      key_masks=kms, hopwise=hopwise, document_ids=doc_ids)
     torch.cuda.synchronize()
-    routs, rlses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms)
+    routs, rlses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids)
     err = max((o.float() - r).abs().max().item() for o, r in zip(outs, routs))
     fin = [torch.isfinite(r) for r in rlses]
     lerr = max(((l - r)[f]).abs().max().item() if f.any() else 0.0 for l, r, f in zip(lses, rlses, fin))
@@ -70,7 +136,7 @@ def case_fwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=Fa
 
 
 def case_bwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=False, window=None, softclamp=0.0,
-             kmask=False, dtype="bf16", seed=0, fused=None, hopwise=False):
+             kmask=False, dtype="bf16", seed=0, fused=None, hopwise=False, docs=None):
     import torch
     from ring_attention_pytorch_b200.ops.fused import emulate_ring_backward, emulate_ring_forward
     from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
@@ -83,13 +149,12 @@ def case_bwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=Fa
     ks = [torch.randn(b, n, hk, d, device="cuda", dtype=dt) for _ in range(world)]
     vs = [torch.randn(b, n, hk, d, device="cuda", dtype=dt) for _ in range(world)]
     dos = [torch.randn(b, n, h, d, device="cuda", dtype=dt) for _ in range(world)]
-    kms = None
-    if kmask:
-        kms = [torch.rand(b, n, device="cuda") > 0.3 for _ in range(world)]
+    doc_ids, kms = _case_docs(docs, b, n, world, layout, kmask, seed)
     outs, lses = emulate_ring_forward(qs, ks, vs, layout=layout, causal=causal, window=window, softclamp=softclamp,
-                                      key_masks=kms, hopwise=hopwise)
+                                      key_masks=kms, hopwise=hopwise, document_ids=doc_ids)
     grads = emulate_ring_backward(qs, ks, vs, outs, lses, dos, layout=layout, causal=causal, window=window,
-                                  softclamp=softclamp, key_masks=kms, fused=fused, hopwise=hopwise)
+                                  softclamp=softclamp, key_masks=kms, fused=fused, hopwise=hopwise,
+                                  document_ids=doc_ids)
     torch.cuda.synchronize()
     # fp32 oracle through autograd
     pm = make_position_map(layout, world, n)
@@ -99,10 +164,13 @@ def case_bwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=Fa
     k_all, v_all = torch.cat(kf, 1), torch.cat(vf, 1)
     k_pos = torch.cat([pm.positions(r, "cuda") for r in range(world)])
     km = None if kms is None else torch.cat(kms, 1)
+    labels = _doc_labels(doc_ids, layout, n) if doc_ids is not None else None
     loss = 0.0
     for r in range(world):
         o = attention_with_positions(qf[r], k_all, v_all, pm.positions(r, "cuda"), k_pos, causal=causal, window=window,
-                                     key_mask=km, softclamp_value=softclamp)
+                                     key_mask=km, softclamp_value=softclamp,
+                                     q_doc=None if labels is None else labels[r],
+                                     k_doc=None if labels is None else torch.cat(labels, 1))
         loss = loss + (o * dos[r].float()).sum()
     loss.backward()
     errs = {"dq": 0.0, "dk": 0.0, "dv": 0.0}
