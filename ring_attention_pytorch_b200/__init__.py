@@ -24,6 +24,10 @@ def __getattr__(name):
         from ring_attention_pytorch_b200.ops import ring_cuda
 
         return getattr(ring_cuda, name)
+    if name in ("ring_flash_attn_fp8", "quantize_fp8"):
+        from ring_attention_pytorch_b200.ops import ring_fp8
+
+        return getattr(ring_fp8, name)
     raise AttributeError(name)
 
 
@@ -40,6 +44,8 @@ __all__ = [
     "ring_flash_attn_",
     "ring_flash_attn_cuda",
     "ring_flash_attn_cuda_",
+    "ring_flash_attn_fp8",
+    "quantize_fp8",
     "tree_attn_decode",
     "flash_attn_forward",
     "flash_attn_backward",

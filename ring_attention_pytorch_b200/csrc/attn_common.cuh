@@ -32,6 +32,19 @@ __device__ __forceinline__ void pos_range(const PosMap& pm, int r, int a, int b,
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// fp8 (e4m3) forward: key order of the V^T operand.
+//
+// Inside each 32-key group, lane quad q (= lane % 4) holds the fp32 S accumulator columns {2q, 2q+1, 8+2q, 9+2q, 16+2q,
+// 17+2q, 24+2q, 25+2q} of its rows, while the e4m3 A operand of m64nNk32 wants columns {4q..4q+3, 16+4q..16+4q+3}.
+// Rather than shuffling P between lanes, the consumer feeds its S values in register order as A columns, and the
+// V^T tile stores at key slot kappa the key v8_key_of_slot(kappa), so that sum_kappa P_A[kappa] V^T[kappa] is
+// sum_key P[key] V[key].  ops/ring_fp8.py mirrors this map for the tests.
+// ------------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int v8_key_of_slot(int kappa) {
+  return (kappa & ~31) + 16 * ((kappa >> 4) & 1) + 8 * ((kappa >> 1) & 1) + 2 * ((kappa >> 2) & 3) + (kappa & 1);
+}
+
 // Mask parameters shared by forward and backward kernels.
 struct MaskCfg {
   int causal;

@@ -18,7 +18,11 @@
 // 1/gridDim of every slot), overlapping the NVLink transfer with the MMAs of earlier hops.  Layout (plain / striped /
 // zig-zag), causal + sliding-window masking, key padding and packed documents are position functions evaluated
 // in-kernel; fully masked tiles are never loaded.
+//
+// attn_fwd_fp8_kernel is the same body on e4m3 operands (head dim 128, forward only, see consumer_role): K and V^T
+// slots written by pack_kv_fp8, both attention matmuls as e4m3 wgmma, bf16 output.
 #include <cstdlib>
+#include <stdexcept>
 
 #include "attn_common.cuh"
 
@@ -109,11 +113,12 @@ __device__ __forceinline__ void init_scan(FwdScan<DOCS>& sc, const AttnFwdParams
 // ------------------------------------------------------------------------------------------------
 // warp 8: TMA producer (all 32 lanes scan tiles, lane 0 issues)
 // ------------------------------------------------------------------------------------------------
-template <int D, bool DOCS>
+// FP8: Q, K and V^T tiles are one 128-byte-wide sub-tile each (e4m3), so every tile is one box of SUB_BYTES.
+template <int D, bool DOCS, bool FP8 = false>
 __device__ __forceinline__ void producer_role(FwdSmem<D>& sm, const AttnFwdParams& p, const CUtensorMap* map_q,
                                               const CUtensorMap* map_kv) {
-  constexpr int NSUB = FwdSmem<D>::NSUB;
-  constexpr uint32_t TILE_BYTES = FwdSmem<D>::TILE_BYTES;
+  constexpr int NSUB = FP8 ? 1 : FwdSmem<D>::NSUB;
+  constexpr uint32_t TILE_BYTES = FP8 ? SUB_BYTES : FwdSmem<D>::TILE_BYTES;
   const int lane = lane_id();
   uint32_t n_slot = 0;
   uint32_t items = 0;
@@ -224,7 +229,14 @@ __device__ __forceinline__ void fetch_role(FwdSmem<D>& sm, const AttnFwdParams& 
 // Every consumer walks the whole tile sequence of the item (also tiles its rows do not need, and items whose second
 // tile lies beyond n_q) so that each K/V stage is released by both warpgroups exactly once, in order.
 // ------------------------------------------------------------------------------------------------
-template <int D, bool BF16, bool DOCS>
+//
+// FP8 (e4m3 Q, K, V^T; BF16 output): S = Q K^T and O += P V^T run as m64n128k32 e4m3 wgmma, 4 k-steps each.  P goes
+// from the S registers into the A operand as e4m3 in register order; the V^T tile's key order (v8_key_of_slot) makes
+// that product right.  The lazy maximum keeps P <= 2^8 = 256, inside e4m3's range (448): the fp8 path relies on that
+// threshold.  q_descale * k_descale is folded into the logit scale of each item, v_descale into the epilogue; the
+// carried O of the hop mode stays unscaled (v_descale is the same for every owner).
+// ------------------------------------------------------------------------------------------------
+template <int D, bool BF16, bool DOCS, bool FP8 = false>
 __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParams& p, const int t) {
   constexpr int NO = D / 2;  // O accumulator registers per thread
   // K-major operands (Q, K): 8-row groups 1024 B apart.  MN-major V (B of P V): d sub-tiles SUB_BYTES apart.
@@ -248,6 +260,13 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
   for (int idx = blockIdx.x; idx < total; idx += gridDim.x) {
     Item it;
     decode_item(p, idx, it);
+    float mul_it = mul, pre_it = pre, v_scale = 1.f;
+    if constexpr (FP8) {
+      const float qk = p.q_descale[it.b * p.heads + it.h] * p.k_descale[it.b * p.kv_heads + it.kvh];
+      if (clamp) pre_it *= qk;
+      else mul_it *= qk;
+      v_scale = p.v_descale[it.b * p.kv_heads + it.kvh];
+    }
     const uint32_t buf = items & 1;
     mbar_wait(&sm.q_full[buf], (items >> 1) & 1, 400 + t);
     items++;
@@ -307,10 +326,16 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
       if (need) {
         const uint64_t k_desc = gmma_desc(kmaj, sm.kv[ks]);
         wgmma_fence();
+        if constexpr (FP8) {
 #pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t off = (kk / 4) * SUB_BYTES + (kk % 4) * 32;
-          wgmma_ss<BF16, 128, 0, 0>(s, gmma_desc_add(q_desc, off), gmma_desc_add(k_desc, off), kk > 0 ? 1u : 0u);
+          for (int kk = 0; kk < D / 32; ++kk)
+            wgmma_e4m3_ss_n128(s, gmma_desc_add(q_desc, kk * 32), gmma_desc_add(k_desc, kk * 32), kk > 0 ? 1u : 0u);
+        } else {
+#pragma unroll
+          for (int kk = 0; kk < D / 16; ++kk) {
+            const uint32_t off = (kk / 4) * SUB_BYTES + (kk % 4) * 32;
+            wgmma_ss<BF16, 128, 0, 0>(s, gmma_desc_add(q_desc, off), gmma_desc_add(k_desc, off), kk > 0 ? 1u : 0u);
+          }
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -323,7 +348,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
       if (need) {
         if (clamp) {
 #pragma unroll
-          for (int i = 0; i < 64; ++i) s[i] = fast_tanh(s[i] * pre) * post;
+          for (int i = 0; i < 64; ++i) s[i] = fast_tanh(s[i] * pre_it) * post;
         }
         if (part) {
           const int c0 = ti.idx * BN;
@@ -358,7 +383,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
         for (int h = 0; h < 2; ++h) {
           cmax[h] = fmaxf(cmax[h], __shfl_xor_sync(0xffffffffu, cmax[h], 1));
           cmax[h] = fmaxf(cmax[h], __shfl_xor_sync(0xffffffffu, cmax[h], 2));
-          cmax[h] *= mul;
+          cmax[h] *= mul_it;
         }
         float m_eff[2];
 #pragma unroll
@@ -379,21 +404,46 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
 #pragma unroll
         for (int i = 0; i < 64; i += 2) {
           const int h = (i >> 1) & 1;
-          const float e0 = fast_exp2(fmaf(s[i], mul, -m_eff[h]));
-          const float e1 = fast_exp2(fmaf(s[i + 1], mul, -m_eff[h]));
+          const float e0 = fast_exp2(fmaf(s[i], mul_it, -m_eff[h]));
+          const float e1 = fast_exp2(fmaf(s[i + 1], mul_it, -m_eff[h]));
           l[h] += e0 + e1;
-          pa[i / 2] = BF16 ? pack_bf16x2(e0, e1) : pack_f16x2(e0, e1);
+          if constexpr (FP8) {
+            s[i] = e0;
+            s[i + 1] = e1;
+          } else {
+            pa[i / 2] = BF16 ? pack_bf16x2(e0, e1) : pack_f16x2(e0, e1);
+          }
+        }
+        if constexpr (FP8) {
+          // A operand of k-step g = S columns [32 g, 32 g + 32) in register order (see v8_key_of_slot)
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            const float* x = s + 16 * g;
+            pa[4 * g + 0] = pack_e4m3x4(x[0], x[1], x[4], x[5]);
+            pa[4 * g + 1] = pack_e4m3x4(x[2], x[3], x[6], x[7]);
+            pa[4 * g + 2] = pack_e4m3x4(x[8], x[9], x[12], x[13]);
+            pa[4 * g + 3] = pack_e4m3x4(x[10], x[11], x[14], x[15]);
+          }
         }
       }
 
       mbar_wait(&sm.kv_full[vs], vph, 420 + t);
       if (need) {
-        const uint64_t v_desc = gmma_desc(vmaj, sm.kv[vs]);
         wgmma_fence();
+        if constexpr (FP8) {
+          const uint64_t vt_desc = gmma_desc(kmaj, sm.kv[vs]);  // V^T: d rows, key slots K-major
 #pragma unroll
-        for (int kk = 0; kk < BN / 16; ++kk) {
-          const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-          wgmma_rs<BF16, D, 1>(o, a4, gmma_desc_add(v_desc, kk * 2048), 1u);
+          for (int kk = 0; kk < BN / 32; ++kk) {
+            const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+            wgmma_e4m3_rs_n128(o, a4, gmma_desc_add(vt_desc, kk * 32), 1u);
+          }
+        } else {
+          const uint64_t v_desc = gmma_desc(vmaj, sm.kv[vs]);
+#pragma unroll
+          for (int kk = 0; kk < BN / 16; ++kk) {
+            const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+            wgmma_rs<BF16, D, 1>(o, a4, gmma_desc_add(v_desc, kk * 2048), 1u);
+          }
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -431,7 +481,8 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (!row_ok[h]) continue;
-      const float inv = l[h] > 0.f ? 1.f / l[h] : 0.f;
+      float inv = l[h] > 0.f ? 1.f / l[h] : 0.f;
+      if constexpr (FP8) inv *= v_scale;
       uint16_t* orow = reinterpret_cast<uint16_t*>(p.o) + (((size_t)it.b * p.n_q + grow[h]) * p.heads + it.h) * D;
 #pragma unroll
       for (int j = 0; j < D / 8; ++j) {
@@ -446,10 +497,9 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
   }
 }
 
-template <int D, bool BF16, bool DOCS>
-__global__ void __launch_bounds__(NTHREADS, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
-                const __grid_constant__ AttnFwdParams p) {
+template <int D, bool BF16, bool DOCS, bool FP8>
+__device__ __forceinline__ void attn_fwd_body(const CUtensorMap& map_q, const CUtensorMap& map_kv,
+                                              const AttnFwdParams& p) {
   extern __shared__ uint8_t smem_raw[];
   FwdSmem<D>& sm =
       *reinterpret_cast<FwdSmem<D>*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -476,14 +526,29 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   if (warp >= 8) {
     setmaxnreg_dec<40>();
     if (warp == 8) {
-      producer_role<D, DOCS>(sm, p, &map_q, &map_kv);
+      producer_role<D, DOCS, FP8>(sm, p, &map_q, &map_kv);
     } else if (warp == 10) {
       if (lane_id() == 0) fetch_role<D>(sm, p);
     }
   } else {
     setmaxnreg_inc<232>();
-    consumer_role<D, BF16, DOCS>(sm, p, warp < 4 ? 0 : 1);
+    consumer_role<D, BF16, DOCS, FP8>(sm, p, warp < 4 ? 0 : 1);
   }
+}
+
+template <int D, bool BF16, bool DOCS>
+__global__ void __launch_bounds__(NTHREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
+                const __grid_constant__ AttnFwdParams p) {
+  attn_fwd_body<D, BF16, DOCS, false>(map_q, map_kv, p);
+}
+
+// e4m3 operands, head dim 128, bf16 output
+template <bool DOCS>
+__global__ void __launch_bounds__(NTHREADS, 1)
+attn_fwd_fp8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
+                    const __grid_constant__ AttnFwdParams p) {
+  attn_fwd_body<128, true, DOCS, true>(map_q, map_kv, p);
 }
 
 }  // namespace
@@ -497,8 +562,12 @@ void launch_attn_fwd(const CUtensorMap& map_q, const CUtensorMap& map_kv, const 
                      cudaStream_t stream) {
   using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnFwdParams);
   // documents are a separate instantiation: the default kernels keep their code unchanged
-  const Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_fwd_kernel<D, true, true> : attn_fwd_kernel<D, false, true>)
-                                           : (p.is_bf16 ? attn_fwd_kernel<D, true, false> : attn_fwd_kernel<D, false, false>);
+  Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_fwd_kernel<D, true, true> : attn_fwd_kernel<D, false, true>)
+                                     : (p.is_bf16 ? attn_fwd_kernel<D, true, false> : attn_fwd_kernel<D, false, false>);
+  if (p.is_fp8) {
+    if (D != 128) throw std::runtime_error("[ring_attention_b200] the fp8 forward needs head dim 128");
+    kern = p.doc_spans != nullptr ? attn_fwd_fp8_kernel<true> : attn_fwd_fp8_kernel<false>;
+  }
   const size_t smem = sizeof(FwdSmem<D>) + 1024;
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
              "attn_fwd smem attribute");

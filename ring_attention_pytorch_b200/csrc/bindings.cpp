@@ -79,22 +79,48 @@ struct FwdHop {
   bool carry_in = false, carry_out = false;
 };
 
+// fp8 forward (attn_fwd_fp8 / attn_fwd_hop_fp8): e4m3 q, uint8 K/V slots of pack_kv_fp8 ([.., 2, b*hk, n_pad, 128]), the
+// true key count and the fp32 descales.
+struct FwdFp8 {
+  int64_t n_k = 0;
+  const Tensor* q_descale = nullptr;
+  const Tensor* k_descale = nullptr;
+  const Tensor* v_descale = nullptr;
+};
+
+const float* descale_ptr(const Tensor& t, int64_t numel, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == numel, name,
+              " must be a contiguous fp32 CUDA tensor of ", numel, " elements");
+  return t.data_ptr<float>();
+}
+
 std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, at::IntArrayRef peer_ptrs,
                                          const c10::optional<Tensor>& ready_opt,
                                          const c10::optional<Tensor>& kmask_bits, int64_t kv_heads, int64_t rank,
                                          bool causal, int64_t window, double scale, double softclamp,
                                          int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                          at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
-                                         const FwdHop& hop, const c10::optional<Tensor>& doc_spans) {
-  check_16bit(q, "q");
-  check_16bit(kv_buf, "kv_buf");
+                                         const FwdHop& hop, const c10::optional<Tensor>& doc_spans,
+                                         const FwdFp8* fp8 = nullptr) {
+  if (fp8 != nullptr) {
+    TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kFloat8_e4m3fn, "q must be a float8_e4m3fn CUDA tensor");
+    TORCH_CHECK(kv_buf.is_cuda() && kv_buf.scalar_type() == at::kByte, "kv_buf must be the uint8 slot of pack_kv_fp8");
+  } else {
+    check_16bit(q, "q");
+    check_16bit(kv_buf, "kv_buf");
+    TORCH_CHECK(kv_buf.scalar_type() == q.scalar_type());
+  }
   const bool hop_mode = hop.owner >= 0;
   TORCH_CHECK(q.dim() == 4 && q.is_contiguous(), "q must be contiguous [b, n, h, d]");
   TORCH_CHECK(kv_buf.dim() == 5 && kv_buf.is_contiguous(), "kv_buf must be contiguous [world, 2, b*hk, n_k, d]");
-  TORCH_CHECK(kv_buf.scalar_type() == q.scalar_type());
   const int b = q.size(0), n_q = q.size(1), h = q.size(2), d = q.size(3);
-  const int world = hop_mode ? hop.world : (int)kv_buf.size(0), n_k = kv_buf.size(3);
+  const int world = hop_mode ? hop.world : (int)kv_buf.size(0);
+  const int n_k = fp8 != nullptr ? (int)fp8->n_k : (int)kv_buf.size(3);
   TORCH_CHECK(kv_buf.size(1) == 2 && kv_buf.size(2) == b * kv_heads && kv_buf.size(4) == d);
+  if (fp8 != nullptr) {
+    TORCH_CHECK(d == 128, "the fp8 forward needs head dim 128");
+    TORCH_CHECK(n_k > 0 && kv_buf.size(3) == (n_k + 127) / 128 * 128, "fp8 kv_buf needs round_up(n_k, 128) key rows");
+  }
   TORCH_CHECK(d == 64 || d == 128, "head dim must be 64 or 128");
   TORCH_CHECK(h % kv_heads == 0);
   TORCH_CHECK(world <= rab::kMaxWorld);
@@ -108,7 +134,7 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
   c10::cuda::CUDAGuard guard(q.device());
   auto stream = at::cuda::getCurrentCUDAStream();
 
-  Tensor o = torch::empty_like(q);
+  Tensor o = fp8 != nullptr ? torch::empty(q.sizes(), q.options().dtype(at::kBFloat16)) : torch::empty_like(q);
   Tensor lse = torch::empty({b, h, n_q}, q.options().dtype(at::kFloat));
 
   rab::AttnFwdParams p;
@@ -132,7 +158,14 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
     p.kmask_words = km.size(2);
   }
   p.doc_spans = doc_spans_ptr(doc_spans, world, b, n_q, n_k, q_pos_offset);
-  p.slot_bytes = 2ull * b * kv_heads * n_k * d * 2;
+  p.slot_bytes = 2ull * b * kv_heads * kv_buf.size(3) * d * kv_buf.element_size();
+  if (fp8 != nullptr) {
+    p.is_fp8 = 1;
+    p.is_bf16 = 1;  // output type
+    p.q_descale = descale_ptr(*fp8->q_descale, (int64_t)b * h, "q_descale");
+    p.k_descale = descale_ptr(*fp8->k_descale, (int64_t)b * kv_heads, "k_descale");
+    p.v_descale = descale_ptr(*fp8->v_descale, (int64_t)b * kv_heads, "v_descale");
+  }
   // the kernels address owner o's K / V at slot o of the buffer; in hop mode the one slot we were given IS slot
   // `owner`, so the base is shifted down by owner slots (only that slot is ever dereferenced)
   uint8_t* kv_base = reinterpret_cast<uint8_t*>(kv_buf.data_ptr()) - (hop_mode ? hop.owner * p.slot_bytes : 0);
@@ -151,6 +184,21 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
     p.fetch_times = (g_fetch_times != nullptr && g_fetch_times_rows >= sm_count()) ? g_fetch_times : nullptr;
   }
 
+  if (fp8 != nullptr) {
+    // Q: [b, n, h, 128] bytes -> dims (d, h, n, b), box (128, 1, 128, 1).  K and V^T tiles are both 128 rows of 128
+    // bytes: dims (128, n_pad, b*hk, 2*world), box (128, 128, 1, 1), K / V^T of tile i at rows [128 i, 128 i + 128)
+    const int n_pad = kv_buf.size(3);
+    uint64_t qdims[4] = {(uint64_t)d, (uint64_t)h, (uint64_t)n_q, (uint64_t)b};
+    uint64_t qstr[3] = {(uint64_t)d, (uint64_t)h * d, (uint64_t)n_q * h * d};
+    uint32_t qbox[4] = {128, 1, 128, 1};
+    CUtensorMap map_q = rab::make_tmap_u8(q.data_ptr(), 4, qdims, qstr, qbox, rab::TmapSwizzle::B128);
+    uint64_t kdims[4] = {(uint64_t)d, (uint64_t)n_pad, (uint64_t)b * kv_heads, (uint64_t)2 * world};
+    uint64_t kstr[3] = {(uint64_t)d, (uint64_t)n_pad * d, (uint64_t)b * kv_heads * n_pad * d};
+    uint32_t kbox[4] = {128, 128, 1, 1};
+    CUtensorMap map_kv = rab::make_tmap_u8(kv_base, 4, kdims, kstr, kbox, rab::TmapSwizzle::B128);
+    rab::launch_attn_fwd<128>(map_q, map_kv, p, sm_count(), stream);
+    return {o, lse};
+  }
   // Q: [b, n, h, d] -> dims (d, h, n, b), box (64, 1, 128, 1)
   uint64_t qdims[4] = {(uint64_t)d, (uint64_t)h, (uint64_t)n_q, (uint64_t)b};
   uint64_t qstr[3] = {(uint64_t)d * 2, (uint64_t)h * d * 2, (uint64_t)n_q * h * d * 2};
@@ -182,13 +230,13 @@ std::tuple<Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& kv_buf, at::I
 
 // One ring hop of the forward: q against owner `owner`'s K / V slot.  carry_o fp32 [b, n_q, h, d] and carry_ml fp32
 // [2, b*h, n_q] hold the online-softmax state between hops; the launch with carry_out = false writes the final O / lse.
-std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, int64_t owner, int64_t world,
-                                        Tensor carry_o, Tensor carry_ml, bool carry_in, bool carry_out,
-                                        const c10::optional<Tensor>& kmask_bits, int64_t kv_heads, int64_t rank,
-                                        bool causal, int64_t window, double scale, double softclamp,
-                                        int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
-                                        at::IntArrayRef base1, int64_t q_pos_offset,
-                                        const c10::optional<Tensor>& doc_spans) {
+std::tuple<Tensor, Tensor> attn_fwd_hop_impl(const Tensor& q, const Tensor& kv_slot, int64_t owner, int64_t world,
+                                             Tensor carry_o, Tensor carry_ml, bool carry_in, bool carry_out,
+                                             const c10::optional<Tensor>& kmask_bits, int64_t kv_heads, int64_t rank,
+                                             bool causal, int64_t window, double scale, double softclamp,
+                                             int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
+                                             at::IntArrayRef base1, int64_t q_pos_offset,
+                                             const c10::optional<Tensor>& doc_spans, const FwdFp8* fp8) {
   TORCH_CHECK(q.dim() == 4);
   const int64_t b = q.size(0), n_q = q.size(1), h = q.size(2), d = q.size(3);
   TORCH_CHECK(carry_o.is_cuda() && carry_o.scalar_type() == at::kFloat && carry_o.is_contiguous() &&
@@ -205,7 +253,47 @@ std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, 
   hop.carry_out = carry_out;
   const int64_t owners[1] = {owner};
   return attn_fwd_impl(q, kv_slot, {}, c10::nullopt, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
-                       pos_stride, seg_len, base0, base1, q_pos_offset, at::IntArrayRef(owners, 1), hop, doc_spans);
+                       pos_stride, seg_len, base0, base1, q_pos_offset, at::IntArrayRef(owners, 1), hop, doc_spans, fp8);
+}
+
+std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, int64_t owner, int64_t world,
+                                        Tensor carry_o, Tensor carry_ml, bool carry_in, bool carry_out,
+                                        const c10::optional<Tensor>& kmask_bits, int64_t kv_heads, int64_t rank,
+                                        bool causal, int64_t window, double scale, double softclamp,
+                                        int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
+                                        at::IntArrayRef base1, int64_t q_pos_offset,
+                                        const c10::optional<Tensor>& doc_spans) {
+  return attn_fwd_hop_impl(q, kv_slot, owner, world, carry_o, carry_ml, carry_in, carry_out, kmask_bits, kv_heads, rank,
+                           causal, window, scale, softclamp, pos_stride, seg_len, base0, base1, q_pos_offset, doc_spans,
+                           nullptr);
+}
+
+// fp8 forward (head dim 128): q e4m3 [b, n_q, h, 128], kv_buf the uint8 [world, 2, b*hk, n_pad, 128] gather of
+// pack_kv_fp8 slots with n_k true keys per owner, descales fp32 [b*h] / [b*hk].  Returns bf16 o and fp32 lse.
+std::tuple<Tensor, Tensor> attn_fwd_fp8(const Tensor& q, const Tensor& kv_buf, int64_t n_k, const Tensor& q_descale,
+                                        const Tensor& k_descale, const Tensor& v_descale, at::IntArrayRef peer_ptrs,
+                                        const Tensor& ready, const c10::optional<Tensor>& kmask_bits,
+                                        int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
+                                        double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
+                                        at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
+                                        const c10::optional<Tensor>& doc_spans) {
+  const FwdFp8 fp8{n_k, &q_descale, &k_descale, &v_descale};
+  return attn_fwd_impl(q, kv_buf, peer_ptrs, ready, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
+                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{}, doc_spans, &fp8);
+}
+
+std::tuple<Tensor, Tensor> attn_fwd_hop_fp8(const Tensor& q, const Tensor& kv_slot, int64_t n_k,
+                                            const Tensor& q_descale, const Tensor& k_descale, const Tensor& v_descale,
+                                            int64_t owner, int64_t world, Tensor carry_o, Tensor carry_ml,
+                                            bool carry_in, bool carry_out, const c10::optional<Tensor>& kmask_bits,
+                                            int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
+                                            double softclamp, int64_t pos_stride, int64_t seg_len,
+                                            at::IntArrayRef base0, at::IntArrayRef base1, int64_t q_pos_offset,
+                                            const c10::optional<Tensor>& doc_spans) {
+  const FwdFp8 fp8{n_k, &q_descale, &k_descale, &v_descale};
+  return attn_fwd_hop_impl(q, kv_slot, owner, world, carry_o, carry_ml, carry_in, carry_out, kmask_bits, kv_heads, rank,
+                           causal, window, scale, softclamp, pos_stride, seg_len, base0, base1, q_pos_offset, doc_spans,
+                           &fp8);
 }
 
 
@@ -576,6 +664,24 @@ void pack_kv(const Tensor& k, const Tensor& v, Tensor slot, int64_t which) {
                       v.stride(0), v.stride(1), v.stride(2), (int)which, at::cuda::getCurrentCUDAStream());
 }
 
+// k, v [b, n, hk, 128] e4m3 (unit stride on d) -> slot uint8 [2, b*hk, n_pad, 128] (layout in kernels.h)
+void pack_kv_fp8(const Tensor& k, const Tensor& v, Tensor slot) {
+  TORCH_CHECK(k.is_cuda() && k.scalar_type() == at::kFloat8_e4m3fn && v.scalar_type() == at::kFloat8_e4m3fn,
+              "k / v must be float8_e4m3fn CUDA tensors");
+  TORCH_CHECK(k.dim() == 4 && k.sizes() == v.sizes() && k.size(3) == 128, "k / v must be [b, n, hk, 128]");
+  TORCH_CHECK(k.stride(3) == 1 && v.stride(3) == 1, "k/v need unit stride on the head dim");
+  for (int i = 0; i < 3; ++i)
+    TORCH_CHECK(k.stride(i) % 16 == 0 && v.stride(i) % 16 == 0, "k/v strides must be multiples of 16 elements");
+  const int b = k.size(0), n = k.size(1), hk = k.size(2);
+  const int64_t n_pad = (n + 127) / 128 * 128;
+  TORCH_CHECK(slot.is_cuda() && slot.scalar_type() == at::kByte && slot.is_contiguous() &&
+                  slot.numel() == 2 * (int64_t)b * hk * n_pad * 128,
+              "slot must be contiguous uint8 [2, b*hk, n_pad, 128]");
+  c10::cuda::CUDAGuard guard(k.device());
+  rab::launch_pack_kv_fp8(k.data_ptr(), v.data_ptr(), slot.data_ptr(), b, n, hk, k.stride(0), k.stride(1), k.stride(2),
+                          v.stride(0), v.stride(1), v.stride(2), at::cuda::getCurrentCUDAStream());
+}
+
 // x [b, n, h, d] 16 bit (unit stride on d) -> out, rotated by angles [n, >= d/2] fp32 (sign -1: inverse rotation).
 //   head_major = false: out [b, n, h, d_out] (d_out >= d: the caller pre-zeroes the padding columns)
 //   head_major = true : out [b*h, n, d_out]  (one half of a K/V gather slot)
@@ -678,6 +784,15 @@ TORCH_LIBRARY(rab, m) {
         "carry_in, bool carry_out, Tensor? kmask_bits, int kv_heads, int rank, bool causal, int window, float scale, "
         "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None) "
         "-> (Tensor, Tensor)");
+  m.def("attn_fwd_fp8(Tensor q, Tensor kv_buf, int n_k, Tensor q_descale, Tensor k_descale, Tensor v_descale, int[] "
+        "peer_ptrs, Tensor ready, Tensor? kmask_bits, int kv_heads, int rank, bool causal, int window, float scale, "
+        "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner, "
+        "Tensor? doc_spans=None) -> (Tensor, Tensor)");
+  m.def("attn_fwd_hop_fp8(Tensor q, Tensor kv_slot, int n_k, Tensor q_descale, Tensor k_descale, Tensor v_descale, int "
+        "owner, int world, Tensor(a!) carry_o, Tensor(b!) carry_ml, bool carry_in, bool carry_out, Tensor? kmask_bits, "
+        "int kv_heads, int rank, bool causal, int window, float scale, float softclamp, int pos_stride, int seg_len, "
+        "int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None) -> (Tensor, Tensor)");
+  m.def("pack_kv_fp8(Tensor k, Tensor v, Tensor(a!) slot) -> ()");
   m.def("acc_convert(Tensor acc, Tensor(a!) out, float scale) -> ()");
   m.def("set_fetch_timing(Tensor? times) -> ()");
   m.def("device_barrier(int[] pad_ptrs, int rank, int epoch) -> ()");
@@ -692,6 +807,9 @@ TORCH_LIBRARY_IMPL(rab, CUDA, m) {
   m.impl("attn_fwd", &attn_fwd);
   m.impl("attn_fwd_hop", &attn_fwd_hop);
   m.impl("pack_kv", &pack_kv);
+  m.impl("attn_fwd_fp8", &attn_fwd_fp8);
+  m.impl("attn_fwd_hop_fp8", &attn_fwd_hop_fp8);
+  m.impl("pack_kv_fp8", &pack_kv_fp8);
   m.impl("rotary", &rotary);
   m.impl("tree_decode", &tree_decode);
   m.impl("bwd_prep", &bwd_prep);

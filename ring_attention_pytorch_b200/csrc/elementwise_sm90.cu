@@ -2,6 +2,7 @@
 // peer-mapped signal pads, and small conversion kernels used by the backward pass.
 #include <cuda_fp16.h>
 
+#include "attn_common.cuh"
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -30,6 +31,45 @@ __global__ void pack_kv_kernel(const uint16_t* __restrict__ k, const uint16_t* _
     const uint16_t* src = which ? v + b * v_sb + row * v_sn + h * v_sh : k + b * k_sb + row * k_sn + h * k_sh;
     const uint4 val = *reinterpret_cast<const uint4*>(src + c * 8);
     reinterpret_cast<uint4*>(slot)[i] = val;
+  }
+}
+
+// fp8 slot for the e4m3 forward (layout in kernels.h).  One block per (128-key tile, b*hk): K rows are copied through,
+// V goes through shared memory and leaves transposed, in the key-slot order of v8_key_of_slot.  Keys past n are zero:
+// e4m3 has NaN encodings and P = 0 times NaN would still poison O.
+__global__ void pack_kv_fp8_kernel(const uint8_t* __restrict__ k, const uint8_t* __restrict__ v,
+                                   uint8_t* __restrict__ slot, int batch, int n, int kv_heads, int n_pad,
+                                   long long k_sb, long long k_sn, long long k_sh, long long v_sb, long long v_sn,
+                                   long long v_sh) {
+  __shared__ __align__(16) uint8_t vt[128][128 + 16];
+  const int tile = blockIdx.x, bh = blockIdx.y;
+  const int b = bh / kv_heads, h = bh % kv_heads;
+  const size_t tile_off = ((size_t)bh * n_pad + (size_t)tile * 128) * 128;
+  uint8_t* kdst = slot + tile_off;
+  uint8_t* vdst = slot + (size_t)batch * kv_heads * n_pad * 128 + tile_off;
+  for (int i = threadIdx.x; i < 128 * 8; i += blockDim.x) {
+    const int r = i / 8, c = i % 8;
+    const long long key = (long long)tile * 128 + r;
+    uint4 kx = make_uint4(0, 0, 0, 0), vx = kx;
+    if (key < n) {
+      kx = *reinterpret_cast<const uint4*>(k + b * k_sb + key * k_sn + h * k_sh + c * 16);
+      vx = *reinterpret_cast<const uint4*>(v + b * v_sb + key * v_sn + h * v_sh + c * 16);
+    }
+    reinterpret_cast<uint4*>(kdst)[i] = kx;
+    *reinterpret_cast<uint4*>(&vt[r][c * 16]) = vx;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 128 * 8; i += blockDim.x) {
+    const int dr = i % 128, c = i / 128;  // key slots [16 c, 16 c + 16) of V^T row dr
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      uint32_t x = 0;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) x |= uint32_t(vt[v8_key_of_slot(16 * c + 4 * j + e)][dr]) << (8 * e);
+      w[j] = x;
+    }
+    reinterpret_cast<uint4*>(vdst + dr * 128)[c] = make_uint4(w[0], w[1], w[2], w[3]);
   }
 }
 
@@ -123,6 +163,17 @@ void launch_pack_kv(const void* k, const void* v, void* slot, int batch, int n, 
       reinterpret_cast<const uint16_t*>(k), reinterpret_cast<const uint16_t*>(v), reinterpret_cast<uint16_t*>(slot),
       batch, n, kv_heads, d, k_sb, k_sn, k_sh, v_sb, v_sn, v_sh, which);
   cuda_check(cudaGetLastError(), "pack_kv launch");
+}
+
+void launch_pack_kv_fp8(const void* k, const void* v, void* slot, int batch, int n, int kv_heads, long long k_sb,
+                        long long k_sn, long long k_sh, long long v_sb, long long v_sn, long long v_sh,
+                        cudaStream_t stream) {
+  const int n_pad = (n + 127) / 128 * 128;
+  if (n_pad == 0 || batch * kv_heads == 0) return;
+  pack_kv_fp8_kernel<<<dim3(n_pad / 128, batch * kv_heads), 256, 0, stream>>>(
+      reinterpret_cast<const uint8_t*>(k), reinterpret_cast<const uint8_t*>(v), reinterpret_cast<uint8_t*>(slot), batch,
+      n, kv_heads, n_pad, k_sb, k_sn, k_sh, v_sb, v_sn, v_sh);
+  cuda_check(cudaGetLastError(), "pack_kv_fp8 launch");
 }
 
 void launch_rotary(const void* x, void* out, const float* angles, int astride, int batch, int n, int heads, int d,

@@ -64,6 +64,12 @@ struct AttnFwdParams {
   int all_ready;     // 1: every slot this launch reads is already complete (no in-kernel fetch, no ready flags)
   // document spans int32 [world][batch][n][2]: [start, end) global positions of each token's document (null = off)
   const int* doc_spans;
+  // fp8 operands (head dim 128): q is e4m3 [b, n_q, h, d], the K/V slots are pack_kv_fp8's [2][b*hk][n_pad * d] bytes,
+  // o is bf16.  S is scaled by q_descale[b*h + h] * k_descale[b*hk + kvh], O by v_descale[b*hk + kvh].
+  int is_fp8;
+  const float* q_descale;
+  const float* k_descale;
+  const float* v_descale;
 };
 
 template <int D>
@@ -195,6 +201,15 @@ void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, c
 void launch_pack_kv(const void* k, const void* v, void* slot, int batch, int n, int kv_heads, int d,
                     long long k_sb, long long k_sn, long long k_sh, long long v_sb, long long v_sn,
                     long long v_sh, int which, cudaStream_t stream);
+// fp8 slot for the e4m3 forward (head dim 128).  k, v [b, n, hk, 128] e4m3 (arbitrary batch/seq/head strides, unit d
+// stride) -> slot [2][b*hk][n_pad * 128] bytes, n_pad = round_up(n, 128):
+//   plane 0: K  [b*hk][n_pad][128]
+//   plane 1: V^T per 128-key tile [b*hk][n_pad / 128][128 (d)][128 (key slot)], slot kappa of a tile holding key
+//            v8_key_of_slot(kappa) (attn_common.cuh)
+// Keys n..n_pad-1 are zero in both planes.
+void launch_pack_kv_fp8(const void* k, const void* v, void* slot, int batch, int n, int kv_heads, long long k_sb,
+                        long long k_sn, long long k_sh, long long v_sb, long long v_sn, long long v_sh,
+                        cudaStream_t stream);
 
 // rotary embedding (rotate-half convention) fused with a layout change; see elementwise_sm90.cu:rotary_kernel
 void launch_rotary(const void* x, void* out, const float* angles, int astride, int batch, int n, int heads, int d,

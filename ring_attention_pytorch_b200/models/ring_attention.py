@@ -257,11 +257,17 @@ class RingAttention(Module):
         rotary_embed: bool = False,
         rotary_embed_theta: int = 10000,
         use_cuda_kernel: Optional[bool] = None,
+        fp8_attn: bool = False,
     ):
+        """``fp8_attn``: forward-only e4m3 attention for inference prefill (call under ``torch.no_grad()``).  q, k and v
+        are quantised with :func:`ring_attention_pytorch_b200.ops.ring_fp8.quantize_fp8` (per-(batch, head) scales over
+        the ring set) and attended with ``ring_flash_attn_fp8``; rotary embedding is applied before the quantisation."""
         super().__init__()
         use_cuda_kernel = default(use_cuda_kernel, cuda_kernels_usable(dim_head))
         assert not (use_cuda_kernel and not torch.cuda.is_available())
         self.use_cuda_kernel = use_cuda_kernel
+        assert not (fp8_attn and force_regular_attn), "fp8_attn runs the ring op, not the regular attention"
+        self.fp8_attn = fp8_attn
 
         self.eps = eps
         self.heads = heads
@@ -336,6 +342,8 @@ class RingAttention(Module):
         q, k, v = qkv.view(b, n, -1, self.dim_head).split(self.qkv_head_breakdown, dim=-2)
 
         use_ring = ring_attn and not force_ring_reduce_off
+        if self.fp8_attn and torch.is_grad_enabled():
+            raise ValueError("RingAttention(fp8_attn=True) is forward only: call it under torch.no_grad()")
         if not exists(rotary_emb) and exists(self.rotary_embed):
             rotary_emb = self.rotary_embed(n, ring_size if use_ring else 1) if use_ring else \
                 self.rotary_embed(torch.arange(n, device=x.device))
@@ -343,7 +351,7 @@ class RingAttention(Module):
         kernel_path = any_cuda_inputs and self.use_cuda_kernel and not self.force_regular_attn
         # On the sm_90a path the rotation of q and k happens inside the op's pack kernels (fp32 sincos from the same
         # angles, fused with the head-major repack): no eager elementwise passes over q and k.
-        fuse_rotary = kernel_path and exists(rotary_emb) and self.dim_head % 16 == 0
+        fuse_rotary = kernel_path and exists(rotary_emb) and self.dim_head % 16 == 0 and not self.fp8_attn
         if exists(rotary_emb) and not fuse_rotary:
             q = apply_rotary_pos_emb(rotary_emb, q)
             k = apply_rotary_pos_emb(rotary_emb, k)
@@ -354,6 +362,16 @@ class RingAttention(Module):
                                            q_doc=runs, k_doc=runs)
         elif self.force_regular_attn:
             out = default_attention(q, k, v, mask=mask, causal=self.causal)
+        elif self.fp8_attn:
+            from ring_attention_pytorch_b200.ops.ring_fp8 import (dequantized_ring_flash_attn, quantize_fp8,
+                                                                  ring_flash_attn_fp8)
+
+            (q8, qd), (k8, kd), (v8, vd) = (quantize_fp8(t, ring_size if use_ring else 1) for t in (q, k, v))
+            args = (mask, self.causal, self.bucket_size, use_ring, self.striped_ring_attn and use_ring,
+                    self.max_lookback_seq_len, ring_size)
+            # off the kernel path the op's definition runs: the portable ring op on the dequantised inputs
+            attn = ring_flash_attn_fp8 if kernel_path else dequantized_ring_flash_attn
+            out = attn(q8, k8, v8, qd, kd, vd, *args, document_ids=document_ids).to(q.dtype)
         elif kernel_path:
             from ring_attention_pytorch_b200.ops.ring_cuda import ring_flash_attn_cuda
 
@@ -402,6 +420,7 @@ class RingTransformer(Module):
         force_regular_attn: bool = False,
         use_cuda_kernel: Optional[bool] = None,
         ff_chunk_size: Optional[int] = None,
+        fp8_attn: bool = False,
     ):
         super().__init__()
         use_cuda_kernel = default(use_cuda_kernel, cuda_kernels_usable(dim_head))
@@ -432,7 +451,7 @@ class RingTransformer(Module):
                               ring_attn=ring_attn, ring_seq_size=ring_seq_size,
                               max_lookback_seq_len=layer_max_lookback_seq_len, striped_ring_attn=striped_ring_attn,
                               force_regular_attn=force_regular_attn, use_cuda_kernel=self.use_cuda_kernel,
-                              auto_shard_seq=False),
+                              auto_shard_seq=False, fp8_attn=fp8_attn),
                 FeedForward(dim=dim, mult=ff_mult, chunk_size=ff_chunk_size),
             ]))
         self.to_logits = nn.Sequential(RMSNorm(dim), nn.Linear(dim, num_tokens, bias=False))

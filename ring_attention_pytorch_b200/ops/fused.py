@@ -161,6 +161,141 @@ def emulate_ring_forward(
     return outs, lses
 
 
+# ------------------------------------------------------------------------------------------------
+# fp8 (e4m3) forward, head dim 128
+# ------------------------------------------------------------------------------------------------
+def alloc_kv_buffer_fp8(world: int, batch: int, kv_heads: int, n_k: int, device) -> torch.Tensor:
+    """``world`` fp8 slots ``[world, 2, b*hk, pad128(n_k), 128]`` uint8 (layout: ``csrc/kernels.h``, pack_kv_fp8)."""
+    return torch.empty(world, 2, batch * kv_heads, pad128(n_k), 128, dtype=torch.uint8, device=device)
+
+
+def pack_kv_fp8(k: torch.Tensor, v: torch.Tensor, slot: torch.Tensor) -> None:
+    """k, v e4m3 ``[b, n, hk, 128]`` -> one fp8 slot ``[2, b*hk, pad128(n), 128]``: K, then V^T per 128-key tile in the
+    key order of :func:`ring_attention_pytorch_b200.ops.ring_fp8.v8_key_of_slot`; keys past ``n`` are zero."""
+    _ext.ops().pack_kv_fp8(k, v, slot)
+
+
+def fused_attn_fwd_fp8(
+    q: torch.Tensor,
+    kv_buf: torch.Tensor,
+    n_k: int,
+    descales,
+    peer_ptrs: Sequence[int],
+    ready: torch.Tensor,
+    kmask_bits: Optional[torch.Tensor],
+    *,
+    kv_heads: int,
+    rank: int,
+    pm: PositionMap,
+    causal: bool,
+    window: Optional[int],
+    scale: float,
+    softclamp: float = 0.0,
+    q_pos_offset: int = 0,
+    hop_owner: Optional[List[int]] = None,
+    doc_spans: Optional[torch.Tensor] = None,
+):
+    """:func:`fused_attn_fwd` on e4m3 operands: ``q`` e4m3 ``[b, n_q, h, 128]``, ``kv_buf`` the fp8 slots of
+    :func:`alloc_kv_buffer_fp8` holding ``n_k`` keys each, ``descales`` = (q [b*h], k [b*hk], v [b*hk]) fp32.
+    Returns bf16 o and the fp32 lse."""
+    if hop_owner is None:
+        hop_owner = ring_hop_owners(pm, rank, causal, window)
+    qd, kd, vd = descales
+    return _ext.ops().attn_fwd_fp8(
+        q, kv_buf, int(n_k), qd, kd, vd, list(peer_ptrs), ready, kmask_bits, kv_heads, rank, bool(causal),
+        int(window or 0), float(scale), float(softclamp), pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset),
+        list(hop_owner), doc_spans)
+
+
+def fused_attn_fwd_hop_fp8(
+    q: torch.Tensor,
+    kv_slot: torch.Tensor,
+    n_k: int,
+    descales,
+    owner: int,
+    world: int,
+    carry_o: torch.Tensor,
+    carry_ml: torch.Tensor,
+    kmask_bits: Optional[torch.Tensor],
+    *,
+    carry_in: bool,
+    carry_out: bool,
+    kv_heads: int,
+    rank: int,
+    pm: PositionMap,
+    causal: bool,
+    window: Optional[int],
+    scale: float,
+    softclamp: float = 0.0,
+    q_pos_offset: int = 0,
+    doc_spans: Optional[torch.Tensor] = None,
+):
+    """:func:`fused_attn_fwd_hop` on e4m3 operands (see :func:`fused_attn_fwd_fp8`).  The carried O is not scaled by
+    ``v_descale`` (it is the same for every owner); the final launch applies it."""
+    qd, kd, vd = descales
+    return _ext.ops().attn_fwd_hop_fp8(
+        q, kv_slot[None], int(n_k), qd, kd, vd, int(owner), int(world), carry_o, carry_ml, bool(carry_in),
+        bool(carry_out), kmask_bits, kv_heads, rank, bool(causal), int(window or 0), float(scale), float(softclamp),
+        pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), doc_spans)
+
+
+def emulate_ring_forward_fp8(
+    qs: Sequence[torch.Tensor],
+    ks: Sequence[torch.Tensor],
+    vs: Sequence[torch.Tensor],
+    q_descales: Sequence[torch.Tensor],
+    k_descale: torch.Tensor,
+    v_descale: torch.Tensor,
+    *,
+    layout: str = "plain",
+    causal: bool = False,
+    window: Optional[int] = None,
+    softclamp: float = 0.0,
+    key_masks: Optional[Sequence[torch.Tensor]] = None,
+    scale: Optional[float] = None,
+    hopwise: bool = False,
+    document_ids: Optional[Sequence[torch.Tensor]] = None,
+):
+    """:func:`emulate_ring_forward` for the fp8 forward: e4m3 shards, per-rank ``q_descales`` ``[b, h]`` and the
+    ring-wide ``k_descale`` / ``v_descale`` ``[b, hk]`` (fp32).  Returns (outs, lses), outs in bf16."""
+    world = len(qs)
+    b, n, h, d = qs[0].shape
+    hk = ks[0].shape[2]
+    dev = qs[0].device
+    pm = make_position_map(layout, world, n)
+    scale = d ** -0.5 if scale is None else scale
+    bufs = [alloc_kv_buffer_fp8(world, b, hk, n, dev) for _ in range(world)]
+    for r in range(world):
+        bufs[r].zero_()
+        pack_kv_fp8(ks[r], vs[r], bufs[r][r])
+    kd, vd = (t.float().expand(b, hk).contiguous() for t in (k_descale, v_descale))
+    kbits = None
+    if key_masks is not None:
+        kbits = pack_key_mask_bits(torch.stack(list(key_masks), 0))
+    spans = None if document_ids is None else document_spans(torch.stack(list(document_ids), 0), pm)
+    outs, lses = [], []
+    for r in range(world):
+        q = qs[r].contiguous()
+        descales = (q_descales[r].float().expand(b, h).contiguous(), kd, vd)
+        if hopwise:
+            carry_o, carry_ml = alloc_fwd_carry(q)
+            hops = ring_hop_owners(pm, r, causal, window)
+            for s_, owner in enumerate(hops):
+                o, lse = fused_attn_fwd_hop_fp8(q, bufs[owner][owner], n, descales, owner, world, carry_o, carry_ml,
+                                                kbits, carry_in=s_ > 0, carry_out=s_ + 1 < len(hops), kv_heads=hk,
+                                                rank=r, pm=pm, causal=causal, window=window, scale=scale,
+                                                softclamp=softclamp, doc_spans=spans)
+        else:
+            ready = torch.zeros(world, dtype=torch.int32, device=dev)
+            peers = [bufs[o][o].data_ptr() for o in range(world)]  # owner o's own slot
+            o, lse = fused_attn_fwd_fp8(q, bufs[r], n, descales, peers, ready, kbits, kv_heads=hk, rank=r, pm=pm,
+                                        causal=causal, window=window, scale=scale, softclamp=softclamp,
+                                        doc_spans=spans)
+        outs.append(o)
+        lses.append(lse)
+    return outs, lses
+
+
 def pad64(n: int) -> int:
     return (n + 63) // 64 * 64
 

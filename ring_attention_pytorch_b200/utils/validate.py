@@ -56,3 +56,27 @@ def check_attention_inputs(q: Tensor, k: Tensor, v: Tensor, mask: Optional[Tenso
         if mask.dtype != torch.bool or mask.dim() != 2 or mask.shape[0] != k.shape[0] or mask.shape[1] != k.shape[sd]:
             raise ValueError(f"{name}: mask must be bool [batch, keys] = [{k.shape[0]}, {k.shape[sd]}], got "
                              f"{mask.dtype} {tuple(mask.shape)}")
+
+
+def check_fp8_attention_inputs(q: Tensor, k: Tensor, v: Tensor, q_descale, k_descale, v_descale,
+                               mask: Optional[Tensor] = None, *, name: str = "attention",
+                               rotary_freqs: Optional[Tensor] = None) -> None:
+    """Inputs of the fp8 forward: e4m3 q / k / v with the shapes of :func:`check_attention_inputs`, fp32 descales
+    ``[b, h]`` (q) and ``[b, hk]`` (k, v) or one element each, nothing that requires grad, no rotary angles."""
+    check_attention_inputs(q, k, v, mask, name=name)
+    for nm, t in (("q", q), ("k", k), ("v", v)):
+        if t.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"{name}: {nm} must be torch.float8_e4m3fn, got {t.dtype}")
+    b, h, hk = q.shape[0], q.shape[2], k.shape[2]
+    for nm, t, heads in (("q_descale", q_descale, h), ("k_descale", k_descale, hk), ("v_descale", v_descale, hk)):
+        if not torch.is_tensor(t) or t.dtype != torch.float32:
+            raise ValueError(f"{name}: {nm} must be a float32 tensor")
+        if t.numel() != 1 and tuple(t.shape) != (b, heads):
+            raise ValueError(f"{name}: {nm} must be [batch, heads] = [{b}, {heads}] or have one element, got "
+                             f"{tuple(t.shape)}")
+        if t.device != q.device:
+            raise ValueError(f"{name}: {nm} must live on {q.device}, got {t.device}")
+    if any(t.requires_grad for t in (q, k, v, q_descale, k_descale, v_descale)):
+        raise ValueError(f"{name}: the fp8 attention is forward only; an input requires grad")
+    if rotary_freqs is not None:
+        raise ValueError(f"{name}: rotary_freqs is not accepted; rotate q and k first, then quantise them")
