@@ -232,9 +232,16 @@ __device__ __forceinline__ void fetch_role(FwdSmem<D>& sm, const AttnFwdParams& 
 //
 // FP8 (e4m3 Q, K, V^T; BF16 output): S = Q K^T and O += P V^T run as m64n128k32 e4m3 wgmma, 4 k-steps each.  P goes
 // from the S registers into the A operand as e4m3 in register order; the V^T tile's key order (v8_key_of_slot) makes
-// that product right.  The lazy maximum keeps P <= 2^8 = 256, inside e4m3's range (448): the fp8 path relies on that
-// threshold.  q_descale * k_descale is folded into the logit scale of each item, v_descale into the epilogue; the
-// carried O of the hop mode stays unscaled (v_descale is the same for every owner).
+// that product right.  The lazy maximum is not used here: against a maximum that is only raised, every key more than
+// about 7 nats below it falls under e4m3's smallest value (2^-9), and with an attention sink that is most of a long
+// row's tail.  Instead each tile's P is taken against that tile's own maximum minus 8 (so P <= 2^8 = 256, inside
+// e4m3's range of 448); the tile maximum used is floored 2^32 below the running maximum, so the reference is never
+// more than 2^40 below it and O and l stay far inside fp32.  O and l are rescaled to the new reference every tile.
+// l sums the e4m3-rounded P, the same values P V multiplies.  Each tile's P V is accumulated into zeroed registers and
+// added to O in fp32: the e4m3 MMA accumulates at reduced precision, and with O as its accumulator a tile that is
+// small against O loses its low bits.  A carried hop state is handed over against the running maximum.  q_descale * k_descale is folded into the logit scale of
+// each item, v_descale into the epilogue; the carried O of the hop mode stays unscaled (v_descale is the same for
+// every owner).
 // ------------------------------------------------------------------------------------------------
 template <int D, bool BF16, bool DOCS, bool FP8 = false>
 __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParams& p, const int t) {
@@ -289,7 +296,8 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
     }
 
     float o[NO];
-    float m_used[2] = {-INFINITY, -INFINITY};
+    float m_used[2] = {-INFINITY, -INFINITY};  // the reference of O and l (FP8: of the last tile)
+    float m_run[2] = {-INFINITY, -INFINITY};   // FP8: the running maximum
     float l[2] = {0.f, 0.f};
 #pragma unroll
     for (int i = 0; i < NO; ++i) o[i] = 0.f;
@@ -300,6 +308,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
         if (!row_ok[h]) continue;
         const size_t mlrow = ((size_t)it.b * p.heads + it.h) * p.n_q + grow[h];
         m_used[h] = p.carry_ml[mlrow];
+        if constexpr (FP8) m_run[h] = m_used[h];
         l[h] = (lane % 4 == 0) ? p.carry_ml[(size_t)p.batch * p.heads * p.n_q + mlrow] : 0.f;
         const float* crow = p.carry_o + (((size_t)it.b * p.n_q + grow[h]) * p.heads + it.h) * D;
 #pragma unroll
@@ -345,6 +354,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
       if (lane == 0) mbar_arrive(&sm.kv_empty[ks]);
 
       uint32_t pa[32];
+      float o_fac[2] = {1.f, 1.f};  // FP8: rescale of O to this tile's reference
       if (need) {
         if (clamp) {
 #pragma unroll
@@ -388,7 +398,18 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
         float m_eff[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (cmax[h] > m_used[h] + 8.f) {  // raise the running max (rare): rescale l and O
+          if constexpr (FP8) {
+            // P of this tile against the tile's own maximum minus 8 (P <= 2^8); that reference is never taken more
+            // than 2^40 below the running maximum (tile maxima are floored 2^32 below it), so O and l stay far inside
+            // fp32.  l follows the new reference here, O when this tile's P V is added (o_fac)
+            if (cmax[h] != -INFINITY) {
+              m_run[h] = fmaxf(m_run[h], cmax[h]);
+              const float ref = fmaxf(cmax[h], m_run[h] - 32.f) - 8.f;
+              o_fac[h] = (m_used[h] == -INFINITY) ? 0.f : fast_exp2(m_used[h] - ref);
+              l[h] *= o_fac[h];
+              m_used[h] = ref;
+            }
+          } else if (cmax[h] > m_used[h] + 8.f) {  // raise the running max (rare): rescale l and O
             const float m_new = fmaxf(m_used[h], cmax[h]);
             const float factor = (m_used[h] == -INFINITY) ? 0.f : fast_exp2(m_used[h] - m_new);
             l[h] *= factor;
@@ -406,16 +427,17 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
           const int h = (i >> 1) & 1;
           const float e0 = fast_exp2(fmaf(s[i], mul_it, -m_eff[h]));
           const float e1 = fast_exp2(fmaf(s[i + 1], mul_it, -m_eff[h]));
-          l[h] += e0 + e1;
           if constexpr (FP8) {
             s[i] = e0;
             s[i + 1] = e1;
           } else {
+            l[h] += e0 + e1;
             pa[i / 2] = BF16 ? pack_bf16x2(e0, e1) : pack_f16x2(e0, e1);
           }
         }
         if constexpr (FP8) {
-          // A operand of k-step g = S columns [32 g, 32 g + 32) in register order (see v8_key_of_slot)
+          // A operand of k-step g = S columns [32 g, 32 g + 32) in register order (see v8_key_of_slot); even words
+          // hold row r_lo, odd words row r_lo + 8.  l sums the rounded P that P V multiplies.
 #pragma unroll
           for (int g = 0; g < 4; ++g) {
             const float* x = s + 16 * g;
@@ -424,6 +446,8 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
             pa[4 * g + 2] = pack_e4m3x4(x[8], x[9], x[12], x[13]);
             pa[4 * g + 3] = pack_e4m3x4(x[10], x[11], x[14], x[15]);
           }
+#pragma unroll
+          for (int w = 0; w < 16; ++w) l[w & 1] += sum_e4m3x4(pa[w]);
         }
       }
 
@@ -431,11 +455,27 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
       if (need) {
         wgmma_fence();
         if constexpr (FP8) {
+          // The e4m3 MMA adds its products into the accumulator at reduced precision, so with O as the accumulator
+          // a tile that is small against O (the tail of a row behind an attention sink) loses its low bits, tile
+          // after tile.  This tile's P V goes into zeroed registers and is added to O in fp32, one half of the
+          // head dim at a time (d rows 64..127 of the V^T tile start 64 * 128 bytes in) to bound register use.
           const uint64_t vt_desc = gmma_desc(kmaj, sm.kv[vs]);  // V^T: d rows, key slots K-major
 #pragma unroll
-          for (int kk = 0; kk < BN / 32; ++kk) {
-            const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-            wgmma_e4m3_rs_n128(o, a4, gmma_desc_add(vt_desc, kk * 32), 1u);
+          for (int half = 0; half < 2; ++half) {
+            float acc[NO / 2];
+#pragma unroll
+            for (int kk = 0; kk < BN / 32; ++kk) {
+              const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+              wgmma_e4m3_rs_n64(acc, a4, gmma_desc_add(vt_desc, half * 64 * 128 + kk * 32), kk > 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(acc);
+#pragma unroll
+            for (int i = 0; i < NO / 2; ++i) {
+              float& oi = o[half * (NO / 2) + i];
+              oi = fmaf(oi, o_fac[(i >> 1) & 1], acc[i]);
+            }
           }
         } else {
           const uint64_t v_desc = gmma_desc(vmaj, sm.kv[vs]);
@@ -444,10 +484,10 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
             const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
             wgmma_rs<BF16, D, 1>(o, a4, gmma_desc_add(v_desc, kk * 2048), 1u);
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs(o);
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(o);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.kv_empty[vs]);
@@ -466,6 +506,19 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (!row_ok[h]) continue;
+        if constexpr (FP8) {
+          // carry O and l against the running maximum, the reference the next launch starts from
+          if (m_used[h] != -INFINITY) {
+            const float factor = fast_exp2(m_used[h] - m_run[h]);
+            l[h] *= factor;
+#pragma unroll
+            for (int j = 0; j < D / 8; ++j) {
+              o[4 * j + 2 * h] *= factor;
+              o[4 * j + 2 * h + 1] *= factor;
+            }
+            m_used[h] = m_run[h];
+          }
+        }
         float* crow = p.carry_o + (((size_t)it.b * p.n_q + grow[h]) * p.heads + it.h) * D;
 #pragma unroll
         for (int j = 0; j < D / 8; ++j)

@@ -399,6 +399,20 @@ __device__ __forceinline__ void wgmma_e4m3_rs_n128(float (&d)[64], const uint32_
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d));
 }
 
+// m64n64k32 e4m3 with A from registers: the first or second half of the n128 form's output columns.
+__device__ __forceinline__ void wgmma_e4m3_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc,
+                                                  uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d));
+}
+
 template <bool BF16, int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   static_assert(N == 8 || N == 16 || N == 64 || N == 128, "wgmma N");
@@ -514,6 +528,31 @@ __device__ __forceinline__ uint32_t pack_e4m3x4(float x0, float x1, float x2, fl
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(x1), "f"(x0));
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(x3), "f"(x2));
   return uint32_t(lo) | (uint32_t(hi) << 16);
+}
+// Sum of the four e4m3 values of a packed word.  Every e4m3 value is exact in f16, and the sum of four of them
+// (exponents 2^-9 .. 2^8, 4 significant bits) is exact in fp32.
+__device__ __forceinline__ float sum_e4m3x4(uint32_t w) {
+  float s;
+  asm("{\n"
+      ".reg .b16 lo, hi, a0, a1, b0, b1;\n"
+      ".reg .b32 x, y;\n"
+      ".reg .f32 f0, f1, f2, f3;\n"
+      "mov.b32 {lo, hi}, %1;\n"
+      "cvt.rn.f16x2.e4m3x2 x, lo;\n"
+      "cvt.rn.f16x2.e4m3x2 y, hi;\n"
+      "mov.b32 {a0, a1}, x;\n"
+      "mov.b32 {b0, b1}, y;\n"
+      "cvt.f32.f16 f0, a0;\n"
+      "cvt.f32.f16 f1, a1;\n"
+      "cvt.f32.f16 f2, b0;\n"
+      "cvt.f32.f16 f3, b1;\n"
+      "add.f32 f0, f0, f1;\n"
+      "add.f32 f2, f2, f3;\n"
+      "add.f32 %0, f0, f2;\n"
+      "}"
+      : "=f"(s)
+      : "r"(w));
+  return s;
 }
 // fp32x2 helpers (two independent scalar operations; sm_90 has no packed fp32 instructions).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {

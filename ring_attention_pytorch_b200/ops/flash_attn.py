@@ -117,7 +117,7 @@ def _kernel_hop_forward(q, k, v, keep, causal, strict, scale, clamp):
     ops.pack_kv(kp, vp, kv[0])
     ready = torch.zeros(1, dtype=torch.int32, device=q.device)
     kbits = pack_key_mask_bits(keep[None]) if keep is not None else None
-    pm = make_position_map("plain", 1, n_k)
+    pm = make_position_map("plain", 1, max(n_q, n_k))  # query rows past n_k must not wrap
     # strict causal (diagonal masked) == causal with every query position shifted down by one
     o, lse = fused_attn_fwd(qp, kv, [0], ready, kbits, kv_heads=hk, rank=0, pm=pm, causal=causal, window=None,
                             scale=scale, softclamp=clamp, q_pos_offset=-1 if (causal and strict) else 0,
@@ -245,7 +245,7 @@ def _kernel_hop_backward(do, q, k, v, o, lse, keep, causal, strict, scale, clamp
     lse_k = torch.where(lse <= _MASKED_BELOW, torch.full_like(lse, float("inf")), lse).contiguous()
     ops.bwd_prep(qp, op, dop, lse_k, qdo, stat, 0)
     kbits = pack_key_mask_bits(keep[None]) if keep is not None else None
-    pm = make_position_map("plain", 1, n_k)
+    pm = make_position_map("plain", 1, max(n_q, n_k))  # query rows past n_k must not wrap
     dq, dk, dv = fused_attn_bwd(qdo, kv, stat, kbits, batch=b, heads=h, kv_heads=hk, rank=0, pm=pm, causal=causal,
                                 window=None, scale=scale, softclamp=clamp,
                                 q_pos_offset=-1 if (causal and strict) else 0)

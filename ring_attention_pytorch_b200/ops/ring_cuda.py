@@ -246,7 +246,8 @@ class RingFlashAttentionCUDAFunction(Function):
             qp, kp, vp = (_pad_head_dim(t, d_pad).contiguous() for t in (q, k, v))
 
         rank = get_rank() % ring_size if use_ring else 0
-        pm = make_position_map(layout, ring_size, n_k)
+        # max(n_q, n_k): a map of n_k rows would wrap query row i >= n_k of a cross-attention to position i - n_k
+        pm = make_position_map(layout, ring_size, max(n_q, n_k))
         q_off = (n_k - n_q) if (cross_attn and causal) else 0
         dev = q.device
         # document masking: the [ring, b, n, 2] interval table, built once here and reused by every launch of the backward
@@ -326,7 +327,7 @@ class RingFlashAttentionCUDAFunction(Function):
         dev = qp.device
         dop = _pad_head_dim(do.to(dt), d_pad).contiguous()
         n_k = kp.shape[1] if use_ring else kv_saved.shape[3]
-        pm = make_position_map(layout, ring_size, n_k)
+        pm = make_position_map(layout, ring_size, max(n_q, n_k))
         hop_owner = ring_hop_owners(pm, rank, causal, window)
 
         ws = None

@@ -110,7 +110,8 @@ def _ring_flash_attn_fp8_cuda(q, k, v, q_descale, k_descale, v_descale, mask, ca
     descales = (q_descale.float().expand(b, h).contiguous(), k_descale.float().expand(b, hk).contiguous(),
                 v_descale.float().expand(b, hk).contiguous())
     rank = get_rank() % ring_size if use_ring else 0
-    pm = make_position_map(layout, ring_size, n_k)
+    # max(n_q, n_k): a map of n_k rows would wrap query row i >= n_k of a cross-attention to position i - n_k
+    pm = make_position_map(layout, ring_size, max(n_q, n_k))
     q_off = (n_k - n_q) if (cross_attn and causal) else 0
     dev = q.device
     spans = ring_document_spans(document_ids.to(dev), pm, use_ring) if exists(document_ids) else None

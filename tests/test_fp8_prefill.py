@@ -5,6 +5,7 @@ GPU tolerance: relative RMS error of ``out`` against the fp32 oracle on the dequ
 only error is the kernel's: P in e4m3, S accumulated from e4m3 products, bf16 output).  Observed on one H100 80GB HBM3
 (700 W power limit) over the single-GPU cases below: 1.6e-2 to 2.67e-2 for fp8, against 3.1e-3 to 4.1e-3 for the bf16
 kernel on the same dequantised inputs (fp8 / bf16 ratio 5.3 to 6.6).  The 3e-2 first guess held, with little margin.
+Since each tile's P is taken against its own maximum and its P V is added to O in fp32: 1.5e-2 to 2.2e-2 (ratio 4.8 to 5.5), same card.
 ``REL_RMS_TOL`` is 5e-2, 1.9x the worst observed value (twice it would be 5.3e-2, past the 5e-2 ceiling set for this
 bound); ``BF16_RATIO_TOL`` is 13, twice the worst observed ratio, so a layout bug cannot hide behind the loose bound.
 """
@@ -299,6 +300,7 @@ ORACLE_CASES = {
     "documents_causal": dict(n=4096, causal=True, docs=True),
     "documents_noncausal_gqa": dict(h=4, hk=2, docs=True),
     "cross_attention_causal": dict(n=700, n_k=1000, causal=True),
+    "cross_attention_causal_more_queries": dict(n=1000, n_k=300, causal=True),
     "cross_attention_kmask": dict(n=300, n_k=1000, kmask=True),
 }
 
