@@ -774,6 +774,32 @@ __global__ void bwd_prep_kernel(const uint16_t* __restrict__ q, const uint16_t* 
   }
 }
 
+// Attention-sink gradient of this rank's rows, from the stat slot bwd_prep has just written (lse*log2e, delta):
+//   dsinks[h] = -sum_{b,i} exp(sinks[h] - lse[b,h,i]) * delta[b,h,i]
+// One CTA per head, a fixed row-to-thread assignment and a fixed reduction tree: no atomics, so the result is bitwise
+// reproducible.  Rows that see no key have delta = 0 (and, without a sink, lse = +inf), so they add 0.
+constexpr int SINK_GRAD_THREADS = 256;
+__global__ void __launch_bounds__(SINK_GRAD_THREADS)
+sink_grad_kernel(const float* __restrict__ stat_slot, const float* __restrict__ sinks, float* __restrict__ dsinks,
+                 int batch, int n, int heads, int n_pad) {
+  const int h = blockIdx.x;
+  const float s2 = sinks[h] * kLog2e;
+  float acc = 0.f;
+  for (int b = 0; b < batch; ++b) {
+    const float* lse2 = stat_slot + ((long long)b * heads + h) * n_pad;
+    const float* delta = lse2 + (long long)batch * heads * n_pad;
+    for (int i = threadIdx.x; i < n; i += SINK_GRAD_THREADS) acc += exp2f(s2 - lse2[i]) * delta[i];
+  }
+  for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+  __shared__ float part[SINK_GRAD_THREADS / 32];
+  if (lane_id() == 0) part[threadIdx.x / 32] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float total = 0.f;
+    for (int w = 0; w < SINK_GRAD_THREADS / 32; ++w) total += part[w];
+    dsinks[h] = -total;
+  }
+}
 
 // fp32 accumulator [rows_outer][n_pad][d] -> 16 bit [b][n][h][d] (rows_outer = b * h), scaled.  One thread = 8 elements.
 template <bool BF16>
@@ -862,9 +888,12 @@ size_t attn_bwd_fused_smem_bytes() { return sizeof(DkvSmem<128>) + 1024; }
 
 void launch_bwd_prep(const void* q, const void* o, const void* dout, const float* lse, void* qdo_slot,
                      float* stat_slot, int batch, int n, int heads, int d, int n_pad, int is_bf16,
-                     cudaStream_t stream) {
+                     cudaStream_t stream, const float* sinks, float* dsinks) {
   const long long threads_total = (long long)batch * n * heads * (d / 8);
-  if (threads_total == 0) return;
+  if (threads_total == 0) {
+    if (sinks != nullptr) cuda_check(cudaMemsetAsync(dsinks, 0, sizeof(float) * heads, stream), "dsinks memset");
+    return;
+  }
   const int threads = 256;
   const long long blocks = (threads_total + threads - 1) / threads;
   auto kern = is_bf16 ? bwd_prep_kernel<true> : bwd_prep_kernel<false>;
@@ -873,6 +902,10 @@ void launch_bwd_prep(const void* q, const void* o, const void* dout, const float
       reinterpret_cast<const uint16_t*>(dout), lse, reinterpret_cast<uint16_t*>(qdo_slot), stat_slot, batch, n, heads,
       d, n_pad);
   cuda_check(cudaGetLastError(), "bwd_prep launch");
+  if (sinks != nullptr) {
+    sink_grad_kernel<<<heads, SINK_GRAD_THREADS, 0, stream>>>(stat_slot, sinks, dsinks, batch, n, heads, n_pad);
+    cuda_check(cudaGetLastError(), "sink_grad launch");
+  }
 }
 
 void launch_acc_convert(const float* acc, void* out, int batch, int heads, int n, int n_pad, int d, float scale,

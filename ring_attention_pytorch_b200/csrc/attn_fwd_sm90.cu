@@ -243,7 +243,16 @@ __device__ __forceinline__ void fetch_role(FwdSmem<D>& sm, const AttnFwdParams& 
 // each item, v_descale into the epilogue; the carried O of the hop mode stays unscaled (v_descale is the same for
 // every owner).
 // ------------------------------------------------------------------------------------------------
-template <int D, bool BF16, bool DOCS, bool FP8 = false>
+//
+// SINK (a separate instantiation, selected by a non-null p.sinks): the row's learned sink logit sigma_h is its initial
+// softmax state, m = sigma_h * log2(e), l = 1, O = 0, in every launch that does not carry a state in (the single launch,
+// and hop 0 of the hop-wise mode), so it is counted exactly once per row; the carry and the epilogue are unchanged.  A
+// row that sees no key ends with out = 0 and lse = sigma_h.  FP8: the running maximum starts at sigma_h too, so P <= 2^8
+// and a reference at most 2^40 below max(sigma_h, key maxima) still hold.  Only a row whose every key weighs less than
+// 2^-32 of the sink meets the floor: its keys are then taken against sigma_h - 40 log2 units and those below 2^-49 of
+// the sink round to zero in e4m3.
+// ------------------------------------------------------------------------------------------------
+template <int D, bool BF16, bool DOCS, bool FP8 = false, bool SINK = false>
 __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParams& p, const int t) {
   constexpr int NO = D / 2;  // O accumulator registers per thread
   // K-major operands (Q, K): 8-row groups 1024 B apart.  MN-major V (B of P V): d sub-tiles SUB_BYTES apart.
@@ -316,6 +325,17 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
           const float2 x = *reinterpret_cast<const float2*>(crow + 8 * j + cq);
           o[4 * j + 2 * h] = x.x;
           o[4 * j + 2 * h + 1] = x.y;
+        }
+      }
+    }
+    if constexpr (SINK) {
+      if (!p.carry_in) {
+        const float sg = p.sinks[it.h] * kLog2e;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          m_used[h] = sg;
+          if constexpr (FP8) m_run[h] = sg;
+          l[h] = (lane % 4 == 0) ? 1.f : 0.f;  // l is summed over the row's 4 lanes at the end
         }
       }
     }
@@ -550,7 +570,7 @@ __device__ __forceinline__ void consumer_role(FwdSmem<D>& sm, const AttnFwdParam
   }
 }
 
-template <int D, bool BF16, bool DOCS, bool FP8>
+template <int D, bool BF16, bool DOCS, bool FP8, bool SINK = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& map_q, const CUtensorMap& map_kv,
                                               const AttnFwdParams& p) {
   extern __shared__ uint8_t smem_raw[];
@@ -585,7 +605,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& map_q, const CU
     }
   } else {
     setmaxnreg_inc<232>();
-    consumer_role<D, BF16, DOCS, FP8>(sm, p, warp < 4 ? 0 : 1);
+    consumer_role<D, BF16, DOCS, FP8, SINK>(sm, p, warp < 4 ? 0 : 1);
   }
 }
 
@@ -604,6 +624,14 @@ attn_fwd_fp8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   attn_fwd_body<128, true, DOCS, true>(map_q, map_kv, p);
 }
 
+// attention sinks: the same bodies with the sink as initial softmax state (the kernels above keep their code)
+template <int D, bool BF16, bool DOCS, bool FP8>
+__global__ void __launch_bounds__(NTHREADS, 1)
+attn_fwd_sink_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
+                     const __grid_constant__ AttnFwdParams p) {
+  attn_fwd_body<D, BF16, DOCS, FP8, true>(map_q, map_kv, p);
+}
+
 }  // namespace
 
 size_t attn_fwd_smem_bytes(int head_dim) {
@@ -620,6 +648,16 @@ void launch_attn_fwd(const CUtensorMap& map_q, const CUtensorMap& map_kv, const 
   if (p.is_fp8) {
     if (D != 128) throw std::runtime_error("[ring_attention_b200] the fp8 forward needs head dim 128");
     kern = p.doc_spans != nullptr ? attn_fwd_fp8_kernel<true> : attn_fwd_fp8_kernel<false>;
+  }
+  if (p.sinks != nullptr) {
+    if (p.is_fp8) {
+      kern = p.doc_spans != nullptr ? attn_fwd_sink_kernel<128, true, true, true>
+                                    : attn_fwd_sink_kernel<128, true, false, true>;
+    } else if (p.doc_spans != nullptr) {
+      kern = p.is_bf16 ? attn_fwd_sink_kernel<D, true, true, false> : attn_fwd_sink_kernel<D, false, true, false>;
+    } else {
+      kern = p.is_bf16 ? attn_fwd_sink_kernel<D, true, false, false> : attn_fwd_sink_kernel<D, false, false, false>;
+    }
   }
   const size_t smem = sizeof(FwdSmem<D>) + 1024;
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),

@@ -94,6 +94,16 @@ const float* descale_ptr(const Tensor& t, int64_t numel, const char* name) {
   return t.data_ptr<float>();
 }
 
+// Attention sinks fp32 [heads] (natural-log logits, by query head), or null: no sink.
+const float* sinks_ptr(const c10::optional<Tensor>& sinks, int64_t heads, const Tensor& like) {
+  if (!sinks.has_value()) return nullptr;
+  const Tensor& t = *sinks;
+  TORCH_CHECK(t.is_cuda() && t.device() == like.device() && t.scalar_type() == at::kFloat && t.is_contiguous() &&
+                  t.dim() == 1 && t.size(0) == heads,
+              "sinks must be a contiguous fp32 CUDA tensor [", heads, "] on the device of q");
+  return t.data_ptr<float>();
+}
+
 std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, at::IntArrayRef peer_ptrs,
                                          const c10::optional<Tensor>& ready_opt,
                                          const c10::optional<Tensor>& kmask_bits, int64_t kv_heads, int64_t rank,
@@ -101,7 +111,7 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
                                          int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                          at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
                                          const FwdHop& hop, const c10::optional<Tensor>& doc_spans,
-                                         const FwdFp8* fp8 = nullptr) {
+                                         const c10::optional<Tensor>& sinks, const FwdFp8* fp8 = nullptr) {
   if (fp8 != nullptr) {
     TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kFloat8_e4m3fn, "q must be a float8_e4m3fn CUDA tensor");
     TORCH_CHECK(kv_buf.is_cuda() && kv_buf.scalar_type() == at::kByte, "kv_buf must be the uint8 slot of pack_kv_fp8");
@@ -158,6 +168,7 @@ std::tuple<Tensor, Tensor> attn_fwd_impl(const Tensor& q, const Tensor& kv_buf, 
     p.kmask_words = km.size(2);
   }
   p.doc_spans = doc_spans_ptr(doc_spans, world, b, n_q, n_k, q_pos_offset);
+  p.sinks = sinks_ptr(sinks, h, q);
   p.slot_bytes = 2ull * b * kv_heads * kv_buf.size(3) * d * kv_buf.element_size();
   if (fp8 != nullptr) {
     p.is_fp8 = 1;
@@ -223,9 +234,9 @@ std::tuple<Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& kv_buf, at::I
                                     int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
                                     double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                     at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
-                                    const c10::optional<Tensor>& doc_spans) {
+                                    const c10::optional<Tensor>& doc_spans, const c10::optional<Tensor>& sinks) {
   return attn_fwd_impl(q, kv_buf, peer_ptrs, ready, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
-                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{}, doc_spans);
+                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{}, doc_spans, sinks);
 }
 
 // One ring hop of the forward: q against owner `owner`'s K / V slot.  carry_o fp32 [b, n_q, h, d] and carry_ml fp32
@@ -236,7 +247,8 @@ std::tuple<Tensor, Tensor> attn_fwd_hop_impl(const Tensor& q, const Tensor& kv_s
                                              bool causal, int64_t window, double scale, double softclamp,
                                              int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                              at::IntArrayRef base1, int64_t q_pos_offset,
-                                             const c10::optional<Tensor>& doc_spans, const FwdFp8* fp8) {
+                                             const c10::optional<Tensor>& doc_spans,
+                                             const c10::optional<Tensor>& sinks, const FwdFp8* fp8) {
   TORCH_CHECK(q.dim() == 4);
   const int64_t b = q.size(0), n_q = q.size(1), h = q.size(2), d = q.size(3);
   TORCH_CHECK(carry_o.is_cuda() && carry_o.scalar_type() == at::kFloat && carry_o.is_contiguous() &&
@@ -253,7 +265,8 @@ std::tuple<Tensor, Tensor> attn_fwd_hop_impl(const Tensor& q, const Tensor& kv_s
   hop.carry_out = carry_out;
   const int64_t owners[1] = {owner};
   return attn_fwd_impl(q, kv_slot, {}, c10::nullopt, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
-                       pos_stride, seg_len, base0, base1, q_pos_offset, at::IntArrayRef(owners, 1), hop, doc_spans, fp8);
+                       pos_stride, seg_len, base0, base1, q_pos_offset, at::IntArrayRef(owners, 1), hop, doc_spans, sinks,
+                       fp8);
 }
 
 std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, int64_t owner, int64_t world,
@@ -262,10 +275,10 @@ std::tuple<Tensor, Tensor> attn_fwd_hop(const Tensor& q, const Tensor& kv_slot, 
                                         bool causal, int64_t window, double scale, double softclamp,
                                         int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                         at::IntArrayRef base1, int64_t q_pos_offset,
-                                        const c10::optional<Tensor>& doc_spans) {
+                                        const c10::optional<Tensor>& doc_spans, const c10::optional<Tensor>& sinks) {
   return attn_fwd_hop_impl(q, kv_slot, owner, world, carry_o, carry_ml, carry_in, carry_out, kmask_bits, kv_heads, rank,
                            causal, window, scale, softclamp, pos_stride, seg_len, base0, base1, q_pos_offset, doc_spans,
-                           nullptr);
+                           sinks, nullptr);
 }
 
 // fp8 forward (head dim 128): q e4m3 [b, n_q, h, 128], kv_buf the uint8 [world, 2, b*hk, n_pad, 128] gather of
@@ -276,10 +289,10 @@ std::tuple<Tensor, Tensor> attn_fwd_fp8(const Tensor& q, const Tensor& kv_buf, i
                                         int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
                                         double softclamp, int64_t pos_stride, int64_t seg_len, at::IntArrayRef base0,
                                         at::IntArrayRef base1, int64_t q_pos_offset, at::IntArrayRef hop_owner,
-                                        const c10::optional<Tensor>& doc_spans) {
+                                        const c10::optional<Tensor>& doc_spans, const c10::optional<Tensor>& sinks) {
   const FwdFp8 fp8{n_k, &q_descale, &k_descale, &v_descale};
   return attn_fwd_impl(q, kv_buf, peer_ptrs, ready, kmask_bits, kv_heads, rank, causal, window, scale, softclamp,
-                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{}, doc_spans, &fp8);
+                       pos_stride, seg_len, base0, base1, q_pos_offset, hop_owner, FwdHop{}, doc_spans, sinks, &fp8);
 }
 
 std::tuple<Tensor, Tensor> attn_fwd_hop_fp8(const Tensor& q, const Tensor& kv_slot, int64_t n_k,
@@ -289,19 +302,21 @@ std::tuple<Tensor, Tensor> attn_fwd_hop_fp8(const Tensor& q, const Tensor& kv_sl
                                             int64_t kv_heads, int64_t rank, bool causal, int64_t window, double scale,
                                             double softclamp, int64_t pos_stride, int64_t seg_len,
                                             at::IntArrayRef base0, at::IntArrayRef base1, int64_t q_pos_offset,
-                                            const c10::optional<Tensor>& doc_spans) {
+                                            const c10::optional<Tensor>& doc_spans,
+                                            const c10::optional<Tensor>& sinks) {
   const FwdFp8 fp8{n_k, &q_descale, &k_descale, &v_descale};
   return attn_fwd_hop_impl(q, kv_slot, owner, world, carry_o, carry_ml, carry_in, carry_out, kmask_bits, kv_heads, rank,
                            causal, window, scale, softclamp, pos_stride, seg_len, base0, base1, q_pos_offset, doc_spans,
-                           &fp8);
+                           sinks, &fp8);
 }
 
 
 // ---------------------------------------------------------------------------------------------
 // fused ring attention backward
 // ---------------------------------------------------------------------------------------------
+// sinks fp32 [h] (optional): also writes dsinks fp32 [h], the sink gradient of this rank's rows
 void bwd_prep(const Tensor& q, const Tensor& o, const Tensor& dout, const Tensor& lse, Tensor qdo_buf,
-              Tensor stat_buf, int64_t rank) {
+              Tensor stat_buf, int64_t rank, const c10::optional<Tensor>& sinks, const c10::optional<Tensor>& dsinks) {
   check_16bit(q, "q");
   TORCH_CHECK(q.is_contiguous() && o.is_contiguous() && dout.is_contiguous() && lse.is_contiguous());
   TORCH_CHECK(o.scalar_type() == q.scalar_type() && dout.scalar_type() == q.scalar_type());
@@ -312,10 +327,18 @@ void bwd_prep(const Tensor& q, const Tensor& o, const Tensor& dout, const Tensor
   TORCH_CHECK(stat_buf.dim() == 4 && stat_buf.is_contiguous() && stat_buf.size(1) == 2 && stat_buf.size(2) == b * h);
   const int n_pad = stat_buf.size(3);
   TORCH_CHECK(n_pad >= n && n_pad % 64 == 0);
+  const float* sk = sinks_ptr(sinks, h, q);
+  float* dsk = nullptr;
+  if (sk != nullptr) {
+    TORCH_CHECK(dsinks.has_value() && dsinks->is_cuda() && dsinks->scalar_type() == at::kFloat &&
+                    dsinks->is_contiguous() && dsinks->numel() == h,
+                "dsinks must be a contiguous fp32 CUDA tensor of ", h, " elements");
+    dsk = dsinks->data_ptr<float>();
+  }
   c10::cuda::CUDAGuard guard(q.device());
   rab::launch_bwd_prep(q.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(),
                        qdo_buf[rank].data_ptr(), stat_buf[rank].data_ptr<float>(), b, n, h, d, n_pad,
-                       q.scalar_type() == at::kBFloat16, at::cuda::getCurrentCUDAStream());
+                       q.scalar_type() == at::kBFloat16, at::cuda::getCurrentCUDAStream(), sk, dsk);
 }
 
 struct BwdSetup {
@@ -551,7 +574,7 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
                  Tensor group_done, Tensor counters, at::IntArrayRef partial_ptrs, int64_t aux_local_ptr,
                  at::IntArrayRef pad_ptrs, int64_t mc_partial_ptr, int64_t mc_aux_ptr, int64_t rank, Tensor out,
                  int64_t kv_heads, int64_t splits, double scale, int64_t scale_block_keys, double eps, int64_t grid,
-                 bool tensor_core) {
+                 bool tensor_core, const c10::optional<Tensor>& sinks) {
   TORCH_CHECK(q.is_cuda() && q.is_contiguous() && q.dim() == 3, "q must be contiguous [b, h, d]");
   const int b = q.size(0), h = q.size(1), d = q.size(2);
   TORCH_CHECK(d == 64 || d == 128, "tree decode supports head dim 64 or 128");
@@ -626,6 +649,7 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   p.out_kind = out.scalar_type() == at::kBFloat16 ? 1 : (out.scalar_type() == at::kHalf ? 0 : 2);
   TORCH_CHECK(p.out_kind != 2 || out.scalar_type() == at::kFloat);
   p.eps = (float)eps;
+  p.sinks = sinks_ptr(sinks, h, q);
   c10::cuda::CUDAGuard guard(q.device());
   if (tensor_core) {
     TORCH_CHECK(d == 128 && n > 0, "the tensor-core decode kernel needs head dim 128 and a non-empty shard");
@@ -759,15 +783,16 @@ void symm_close(int64_t ptr) { rab::symm_close(reinterpret_cast<void*>(ptr)); }
 TORCH_LIBRARY(rab, m) {
   m.def("attn_fwd(Tensor q, Tensor kv_buf, int[] peer_ptrs, Tensor ready, Tensor? kmask_bits, int kv_heads, int rank, "
         "bool causal, int window, float scale, float softclamp, int pos_stride, int seg_len, int[] base0, int[] "
-        "base1, int q_pos_offset, int[] hop_owner, Tensor? doc_spans=None) -> (Tensor, Tensor)");
+        "base1, int q_pos_offset, int[] hop_owner, Tensor? doc_spans=None, Tensor? sinks=None) -> (Tensor, Tensor)");
   m.def("pack_kv(Tensor k, Tensor v, Tensor(a!) slot, int which=3) -> ()");
   m.def("rotary(Tensor x, Tensor angles, Tensor(a!) out, bool head_major, float sign) -> ()");
   m.def("tree_decode(Tensor q, Tensor? k, Tensor? v, Tensor? k_scale, Tensor? v_scale, Tensor(a!) scratch, Tensor(b!) "
         "group_done, Tensor(c!) counters, int[] partial_ptrs, int aux_local_ptr, int[] pad_ptrs, int mc_partial_ptr, int "
         "mc_aux_ptr, int rank, Tensor(d!) out, int kv_heads, int splits, float scale, int scale_block_keys, float eps, "
-        "int grid, bool tensor_core) -> ()");
+        "int grid, bool tensor_core, Tensor? sinks=None) -> ()");
   m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core) -> int");
-  m.def("bwd_prep(Tensor q, Tensor o, Tensor dout, Tensor lse, Tensor(a!) qdo_buf, Tensor(b!) stat_buf, int rank) -> ()");
+  m.def("bwd_prep(Tensor q, Tensor o, Tensor dout, Tensor lse, Tensor(a!) qdo_buf, Tensor(b!) stat_buf, int rank, "
+        "Tensor? sinks=None, Tensor(c!)? dsinks=None) -> ()");
   m.def("attn_bwd_dq(Tensor qdo_buf, Tensor kv_buf, Tensor stat_buf, Tensor? ready, int ready_target, Tensor? "
         "kmask_bits, int batch, int heads, int kv_heads, int rank, bool causal, int window, float scale, float "
         "softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner, Tensor? "
@@ -782,16 +807,16 @@ TORCH_LIBRARY(rab, m) {
         "dkv_acc_ptrs, int nk_pad, int world_size=0, int slot_owner=-1, Tensor? doc_spans=None) -> (Tensor, Tensor)");
   m.def("attn_fwd_hop(Tensor q, Tensor kv_slot, int owner, int world, Tensor(a!) carry_o, Tensor(b!) carry_ml, bool "
         "carry_in, bool carry_out, Tensor? kmask_bits, int kv_heads, int rank, bool causal, int window, float scale, "
-        "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None) "
-        "-> (Tensor, Tensor)");
+        "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None, "
+        "Tensor? sinks=None) -> (Tensor, Tensor)");
   m.def("attn_fwd_fp8(Tensor q, Tensor kv_buf, int n_k, Tensor q_descale, Tensor k_descale, Tensor v_descale, int[] "
         "peer_ptrs, Tensor ready, Tensor? kmask_bits, int kv_heads, int rank, bool causal, int window, float scale, "
         "float softclamp, int pos_stride, int seg_len, int[] base0, int[] base1, int q_pos_offset, int[] hop_owner, "
-        "Tensor? doc_spans=None) -> (Tensor, Tensor)");
+        "Tensor? doc_spans=None, Tensor? sinks=None) -> (Tensor, Tensor)");
   m.def("attn_fwd_hop_fp8(Tensor q, Tensor kv_slot, int n_k, Tensor q_descale, Tensor k_descale, Tensor v_descale, int "
         "owner, int world, Tensor(a!) carry_o, Tensor(b!) carry_ml, bool carry_in, bool carry_out, Tensor? kmask_bits, "
         "int kv_heads, int rank, bool causal, int window, float scale, float softclamp, int pos_stride, int seg_len, "
-        "int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None) -> (Tensor, Tensor)");
+        "int[] base0, int[] base1, int q_pos_offset, Tensor? doc_spans=None, Tensor? sinks=None) -> (Tensor, Tensor)");
   m.def("pack_kv_fp8(Tensor k, Tensor v, Tensor(a!) slot) -> ()");
   m.def("acc_convert(Tensor acc, Tensor(a!) out, float scale) -> ()");
   m.def("set_fetch_timing(Tensor? times) -> ()");

@@ -70,6 +70,9 @@ struct AttnFwdParams {
   const float* q_descale;
   const float* k_descale;
   const float* v_descale;
+  // learned attention sinks fp32 [h] (natural-log logits, by query head), null = off: one extra logit per row with a
+  // zero value vector, the row's initial softmax state in every launch that does not carry one in
+  const float* sinks;
 };
 
 template <int D>
@@ -153,9 +156,11 @@ void launch_acc_convert(const float* acc, void* out, int batch, int heads, int n
 
 // q, o, do: [b, n, h, d] contiguous 16 bit; lse: [b, h, n] fp32 (natural log).
 // Writes this rank's slot: qdo_slot [2][b*h][n][d] (q, do) and stat_slot [2][b*h][n_pad] (lse*log2e, delta).
+// sinks fp32 [h] (may be null): also writes dsinks fp32 [h] = -sum_{b,i} exp(sinks[h] - lse) * delta over this rank's
+// rows, reduced in a fixed order (bitwise reproducible).
 void launch_bwd_prep(const void* q, const void* o, const void* dout, const float* lse, void* qdo_slot,
                      float* stat_slot, int batch, int n, int heads, int d, int n_pad, int is_bf16,
-                     cudaStream_t stream);
+                     cudaStream_t stream, const float* sinks = nullptr, float* dsinks = nullptr);
 
 // ------------------------------------------------------------------------------------------------
 // tree-attention decode (tree_decode_sm90.cu): ONE persistent cooperative kernel per rank and step
@@ -185,6 +190,8 @@ struct TreeDecodeParams {
   void* out;                          // [b*h][d]; out_kind 0 fp16, 1 bf16, 2 fp32
   int out_kind;
   float eps;
+  const float* sinks;                 // null or fp32 [heads] attention sinks (natural log, by query head): added once,
+                                      // in the cross-rank merge; the per-rank partials never contain them
 };
 int tree_decode_max_ctas(int d, int kv_kind, int num_sms);
 void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream);

@@ -147,6 +147,8 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
     }
   };
   const bool own = lane * 4 < D;  // one warp per row; lane c owns columns [4c, 4c + 4)
+  // attention sink of row bh in log2 units: one more term of the merged denominator, with a zero value vector
+  auto sink2 = [&](int bh) { return p.sinks[bh % p.heads] * 1.4426950408889634f; };
   if (!nvls) {
     // P2P: every rank reads every peer's row straight over NVLink
     for (int bh = gwarp; bh < rows; bh += nwarps) {
@@ -157,8 +159,10 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
         lse[r] = (p.partials[r] + half_off)[(size_t)bh * row_stride + D];
         mx = fmaxf(mx, lse[r]);
       }
+      const float sg = p.sinks != nullptr ? sink2(bh) : -INFINITY;
+      mx = fmaxf(mx, sg);
       const float m_eff = mx == -INFINITY ? 0.f : mx;
-      float den = 0.f;
+      float den = p.sinks != nullptr ? fast_exp2(sg - m_eff) : 0.f;
       float4 num = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 1
       for (int r = 0; r < p.world; ++r) {
@@ -178,10 +182,13 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
   } else {
     // NVLS: the switch returns M = max_r lse_r (integer max of the order-preserving image); every rank rescales ITS
     // rows in place by w_r = 2^(lse_r - M) and publishes w_r; after a second signal round the switch returns
-    // sum_r w_r out_r and sum_r w_r.
+    // sum_r w_r out_r and sum_r w_r.  With sinks every rank raises M to max(M, sink) first, and rank 0 publishes
+    // w_0 + 2^(sink - M), so the summed denominator holds the sink exactly once.
     const int* mc_ord = reinterpret_cast<const int*>(p.mc_aux + aux_off);
     for (int bh = gwarp; bh < rows; bh += nwarps) {
-      const float M = ordered_to_float(multimem_max_s32(mc_ord + bh));
+      float M = ordered_to_float(multimem_max_s32(mc_ord + bh));
+      const float sg = p.sinks != nullptr ? sink2(bh) : -INFINITY;
+      M = fmaxf(M, sg);
       const float m_eff = M == -INFINITY ? 0.f : M;
       float* row = my_partial + (size_t)bh * row_stride;
       const float l = row[D];
@@ -191,7 +198,7 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
         x.x *= wgt; x.y *= wgt; x.z *= wgt; x.w *= wgt;
         reinterpret_cast<float4*>(row)[lane] = x;
       }
-      if (lane == 0) my_w[bh] = wgt;
+      if (lane == 0) my_w[bh] = (p.sinks != nullptr && p.rank == 0) ? wgt + fast_exp2(sg - m_eff) : wgt;
     }
     __threadfence();
     grid_barrier(&ctr[1], &ctr[2]);

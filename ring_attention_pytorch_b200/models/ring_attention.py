@@ -258,10 +258,15 @@ class RingAttention(Module):
         rotary_embed_theta: int = 10000,
         use_cuda_kernel: Optional[bool] = None,
         fp8_attn: bool = False,
+        attn_sinks: bool = False,
     ):
         """``fp8_attn``: forward-only e4m3 attention for inference prefill (call under ``torch.no_grad()``).  q, k and v
         are quantised with :func:`ring_attention_pytorch_b200.ops.ring_fp8.quantize_fp8` (per-(batch, head) scales over
-        the ring set) and attended with ``ring_flash_attn_fp8``; rotary embedding is applied before the quantisation."""
+        the ring set) and attended with ``ring_flash_attn_fp8``; rotary embedding is applied before the quantisation.
+
+        ``attn_sinks``: a learned attention sink per query head, the parameter ``sinks`` ``[heads]`` (initialised to
+        zero), which every attention path honours (see :func:`ring_attention_pytorch_b200.ops.ring_flash_naive.
+        ring_flash_attn`).  Without it the module has no such parameter, so checkpoints without sinks load unchanged."""
         super().__init__()
         use_cuda_kernel = default(use_cuda_kernel, cuda_kernels_usable(dim_head))
         assert not (use_cuda_kernel and not torch.cuda.is_available())
@@ -304,6 +309,7 @@ class RingAttention(Module):
             nn.Linear(dim, dim_inner + (dim_kv_inner * 2), bias=False),
         )
         self.to_out = nn.Linear(dim_inner, dim, bias=False)
+        self.sinks = nn.Parameter(torch.zeros(heads)) if attn_sinks else None
 
     def forward(
         self,
@@ -356,10 +362,11 @@ class RingAttention(Module):
             q = apply_rotary_pos_emb(rotary_emb, q)
             k = apply_rotary_pos_emb(rotary_emb, k)
 
-        if self.force_regular_attn and exists(document_ids):
-            runs = document_runs(document_ids)
+        sinks = self.sinks
+        if self.force_regular_attn and (exists(document_ids) or exists(sinks)):
+            runs = document_runs(document_ids) if exists(document_ids) else None
             out = attention_with_positions(q, k, v, causal=self.causal, key_mask=None if self.causal else mask,
-                                           q_doc=runs, k_doc=runs)
+                                           q_doc=runs, k_doc=runs, sinks=sinks)
         elif self.force_regular_attn:
             out = default_attention(q, k, v, mask=mask, causal=self.causal)
         elif self.fp8_attn:
@@ -371,17 +378,19 @@ class RingAttention(Module):
                     self.max_lookback_seq_len, ring_size)
             # off the kernel path the op's definition runs: the portable ring op on the dequantised inputs
             attn = ring_flash_attn_fp8 if kernel_path else dequantized_ring_flash_attn
-            out = attn(q8, k8, v8, qd, kd, vd, *args, document_ids=document_ids).to(q.dtype)
+            out = attn(q8, k8, v8, qd, kd, vd, *args, document_ids=document_ids,
+                       sinks=sinks.detach() if exists(sinks) else None).to(q.dtype)
         elif kernel_path:
             from ring_attention_pytorch_b200.ops.ring_cuda import ring_flash_attn_cuda
 
             out = ring_flash_attn_cuda(q, k, v, mask, self.causal, self.bucket_size, use_ring,
                                        self.striped_ring_attn and use_ring, self.max_lookback_seq_len, ring_size,
-                                       rotary_freqs=rotary_emb if fuse_rotary else None, document_ids=document_ids)
+                                       rotary_freqs=rotary_emb if fuse_rotary else None, document_ids=document_ids,
+                                       sinks=sinks)
         else:
             out = ring_flash_attn(q, k, v, mask, self.causal, self.bucket_size, use_ring,
                                   self.striped_ring_attn and use_ring, self.max_lookback_seq_len, ring_size,
-                                  document_ids=document_ids)
+                                  document_ids=document_ids, sinks=sinks)
 
         out = out.reshape(b, n, -1)
         out = self.to_out(out)
@@ -421,7 +430,9 @@ class RingTransformer(Module):
         use_cuda_kernel: Optional[bool] = None,
         ff_chunk_size: Optional[int] = None,
         fp8_attn: bool = False,
+        attn_sinks: bool = False,
     ):
+        """``attn_sinks``: a learned attention sink per query head in every layer (see :class:`RingAttention`)."""
         super().__init__()
         use_cuda_kernel = default(use_cuda_kernel, cuda_kernels_usable(dim_head))
         self.use_cuda_kernel = use_cuda_kernel
@@ -451,7 +462,7 @@ class RingTransformer(Module):
                               ring_attn=ring_attn, ring_seq_size=ring_seq_size,
                               max_lookback_seq_len=layer_max_lookback_seq_len, striped_ring_attn=striped_ring_attn,
                               force_regular_attn=force_regular_attn, use_cuda_kernel=self.use_cuda_kernel,
-                              auto_shard_seq=False, fp8_attn=fp8_attn),
+                              auto_shard_seq=False, fp8_attn=fp8_attn, attn_sinks=attn_sinks),
                 FeedForward(dim=dim, mult=ff_mult, chunk_size=ff_chunk_size),
             ]))
         self.to_logits = nn.Sequential(RMSNorm(dim), nn.Linear(dim, num_tokens, bias=False))

@@ -8,6 +8,10 @@ multi-hop fetch/ready-flag protocol be tested on a single GPU.
 
 ``doc_spans`` (every wrapper) is the int32 ``[world, b, n, 2]`` document interval table of
 :mod:`ring_attention_pytorch_b200.parallel.documents`; ``None`` launches the kernels without document masking.
+
+``sinks`` (the forwards) is the contiguous fp32 ``[h]`` tensor of learned attention sinks, one logit per query head
+that joins every row's softmax denominator with a zero value vector; ``None`` launches the kernels without sinks.
+The forward counts it in the launch that starts a row (the single launch, or hop 0 of the hop-wise mode).
 """
 from __future__ import annotations
 
@@ -55,12 +59,14 @@ def fused_attn_fwd(
     q_pos_offset: int = 0,
     hop_owner: Optional[List[int]] = None,
     doc_spans: Optional[torch.Tensor] = None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     if hop_owner is None:
         hop_owner = ring_hop_owners(pm, rank, causal, window)
     return _ext.ops().attn_fwd(
         q, kv_buf, list(peer_ptrs), ready, kmask_bits, kv_heads, rank, bool(causal), int(window or 0), float(scale),
-        float(softclamp), pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), list(hop_owner), doc_spans)
+        float(softclamp), pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), list(hop_owner), doc_spans,
+        sinks)
 
 
 def fused_attn_fwd_hop(
@@ -83,6 +89,7 @@ def fused_attn_fwd_hop(
     softclamp: float = 0.0,
     q_pos_offset: int = 0,
     doc_spans: Optional[torch.Tensor] = None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     """ONE ring hop of the forward (``memory="ring"``): ``q`` against owner ``owner``'s K/V slot ``[2, b*hk, n_k, d]``.
 
@@ -93,7 +100,7 @@ def fused_attn_fwd_hop(
     return _ext.ops().attn_fwd_hop(
         q, kv_slot[None], int(owner), int(world), carry_o, carry_ml, bool(carry_in), bool(carry_out), kmask_bits,
         kv_heads, rank, bool(causal), int(window or 0), float(scale), float(softclamp), pm.stride, pm.seg_len, pm.base0,
-        pm.base1, int(q_pos_offset), doc_spans)
+        pm.base1, int(q_pos_offset), doc_spans, sinks)
 
 
 def alloc_fwd_carry(q: torch.Tensor):
@@ -115,12 +122,14 @@ def emulate_ring_forward(
     scale: Optional[float] = None,
     hopwise: bool = False,
     document_ids: Optional[Sequence[torch.Tensor]] = None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     """Run the fused forward for every rank of a W-rank ring on the current device.
 
     qs/ks/vs: per-rank shards ``[b, n, h, d]`` / ``[b, n, hk, d]``.  Returns (outs, lses) lists.
     ``hopwise``: one launch per hop with carried softmax state (the ``memory="ring"`` schedule).
     ``document_ids``: per-rank ``[b, n]`` document ids (in the ring's layout) for document masking.
+    ``sinks``: fp32 ``[h]`` attention sinks.
     """
     ops = _ext.ops()
     world = len(qs)
@@ -147,7 +156,7 @@ def emulate_ring_forward(
                 o, lse = fused_attn_fwd_hop(q, bufs[owner][owner], owner, world, carry_o, carry_ml, kbits,
                                             carry_in=s_ > 0, carry_out=s_ + 1 < len(hops), kv_heads=hk, rank=r, pm=pm,
                                             causal=causal, window=window, scale=scale, softclamp=softclamp,
-                                            doc_spans=spans)
+                                            doc_spans=spans, sinks=sinks)
             outs.append(o)
             lses.append(lse)
         return outs, lses
@@ -155,7 +164,8 @@ def emulate_ring_forward(
         ready = torch.zeros(world, dtype=torch.int32, device=dev)
         peers = [bufs[o][o].data_ptr() for o in range(world)]  # owner o's own slot
         o, lse = fused_attn_fwd(qs[r].contiguous(), bufs[r], peers, ready, kbits, kv_heads=hk, rank=r, pm=pm,
-                                causal=causal, window=window, scale=scale, softclamp=softclamp, doc_spans=spans)
+                                causal=causal, window=window, scale=scale, softclamp=softclamp, doc_spans=spans,
+                                sinks=sinks)
         outs.append(o)
         lses.append(lse)
     return outs, lses
@@ -194,6 +204,7 @@ def fused_attn_fwd_fp8(
     q_pos_offset: int = 0,
     hop_owner: Optional[List[int]] = None,
     doc_spans: Optional[torch.Tensor] = None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     """:func:`fused_attn_fwd` on e4m3 operands: ``q`` e4m3 ``[b, n_q, h, 128]``, ``kv_buf`` the fp8 slots of
     :func:`alloc_kv_buffer_fp8` holding ``n_k`` keys each, ``descales`` = (q [b*h], k [b*hk], v [b*hk]) fp32.
@@ -204,7 +215,7 @@ def fused_attn_fwd_fp8(
     return _ext.ops().attn_fwd_fp8(
         q, kv_buf, int(n_k), qd, kd, vd, list(peer_ptrs), ready, kmask_bits, kv_heads, rank, bool(causal),
         int(window or 0), float(scale), float(softclamp), pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset),
-        list(hop_owner), doc_spans)
+        list(hop_owner), doc_spans, sinks)
 
 
 def fused_attn_fwd_hop_fp8(
@@ -229,6 +240,7 @@ def fused_attn_fwd_hop_fp8(
     softclamp: float = 0.0,
     q_pos_offset: int = 0,
     doc_spans: Optional[torch.Tensor] = None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     """:func:`fused_attn_fwd_hop` on e4m3 operands (see :func:`fused_attn_fwd_fp8`).  The carried O is not scaled by
     ``v_descale`` (it is the same for every owner); the final launch applies it."""
@@ -236,7 +248,7 @@ def fused_attn_fwd_hop_fp8(
     return _ext.ops().attn_fwd_hop_fp8(
         q, kv_slot[None], int(n_k), qd, kd, vd, int(owner), int(world), carry_o, carry_ml, bool(carry_in),
         bool(carry_out), kmask_bits, kv_heads, rank, bool(causal), int(window or 0), float(scale), float(softclamp),
-        pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), doc_spans)
+        pm.stride, pm.seg_len, pm.base0, pm.base1, int(q_pos_offset), doc_spans, sinks)
 
 
 def emulate_ring_forward_fp8(
@@ -255,6 +267,7 @@ def emulate_ring_forward_fp8(
     scale: Optional[float] = None,
     hopwise: bool = False,
     document_ids: Optional[Sequence[torch.Tensor]] = None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     """:func:`emulate_ring_forward` for the fp8 forward: e4m3 shards, per-rank ``q_descales`` ``[b, h]`` and the
     ring-wide ``k_descale`` / ``v_descale`` ``[b, hk]`` (fp32).  Returns (outs, lses), outs in bf16."""
@@ -284,13 +297,13 @@ def emulate_ring_forward_fp8(
                 o, lse = fused_attn_fwd_hop_fp8(q, bufs[owner][owner], n, descales, owner, world, carry_o, carry_ml,
                                                 kbits, carry_in=s_ > 0, carry_out=s_ + 1 < len(hops), kv_heads=hk,
                                                 rank=r, pm=pm, causal=causal, window=window, scale=scale,
-                                                softclamp=softclamp, doc_spans=spans)
+                                                softclamp=softclamp, doc_spans=spans, sinks=sinks)
         else:
             ready = torch.zeros(world, dtype=torch.int32, device=dev)
             peers = [bufs[o][o].data_ptr() for o in range(world)]  # owner o's own slot
             o, lse = fused_attn_fwd_fp8(q, bufs[r], n, descales, peers, ready, kbits, kv_heads=hk, rank=r, pm=pm,
                                         causal=causal, window=window, scale=scale, softclamp=softclamp,
-                                        doc_spans=spans)
+                                        doc_spans=spans, sinks=sinks)
         outs.append(o)
         lses.append(lse)
     return outs, lses
@@ -404,9 +417,11 @@ def emulate_ring_backward(
     fused: Optional[bool] = None,
     hopwise: bool = False,
     document_ids=None,
+    sinks: Optional[torch.Tensor] = None,
 ):
     """Backward of :func:`emulate_ring_forward` for every emulated rank on the current device.
     ``hopwise`` (fused only): one launch per hop against a single K/V slot (the ``memory="ring"`` schedule).
+    ``sinks`` (fp32 ``[h]``): every rank's tuple gains a fourth entry, that rank's fp32 sink gradient ``[h]``.
 
     ``fused`` (default: head dim 128) selects the one-kernel backward: every emulated rank adds its dK / dV tiles into
     the owners' fp32 accumulators, exactly what the ranks of a real ring do over NVLink."""
@@ -420,10 +435,11 @@ def emulate_ring_backward(
     kv_all = alloc_kv_buffer(world, b, hk, n, d, dt, dev)
     qdo_all = alloc_qdo_buffer(world, b, h, n, d, dt, dev)
     stat_all = alloc_stat_buffer(world, b, h, n, dev)
+    dsinks = [None if sinks is None else torch.empty(h, dtype=torch.float32, device=dev) for _ in range(world)]
     for r in range(world):
         ops.pack_kv(ks[r], vs[r], kv_all[r])
         ops.bwd_prep(qs[r].contiguous(), outs[r].contiguous(), douts[r].contiguous(), lses[r].contiguous(), qdo_all,
-                     stat_all, r)
+                     stat_all, r, sinks, dsinks[r])
     kbits = None
     if key_masks is not None:
         kbits = pack_key_mask_bits(torch.stack(list(key_masks), 0))
@@ -464,9 +480,11 @@ def emulate_ring_backward(
             else:
                 dk, dv = direct[r]
             res.append((dq, dk, dv))
-        return res
-    for r in range(world):
-        # every emulated rank sees the same fully gathered buffers (what the NVLink gather produces)
-        res.append(fused_attn_bwd(qdo_all, kv_all, stat_all, kbits, batch=b, heads=h, kv_heads=hk, rank=r, pm=pm,
-                                  causal=causal, window=window, scale=scale, softclamp=softclamp, doc_spans=spans))
+    else:
+        for r in range(world):
+            # every emulated rank sees the same fully gathered buffers (what the NVLink gather produces)
+            res.append(fused_attn_bwd(qdo_all, kv_all, stat_all, kbits, batch=b, heads=h, kv_heads=hk, rank=r, pm=pm,
+                                      causal=causal, window=window, scale=scale, softclamp=softclamp, doc_spans=spans))
+    if sinks is not None:
+        res = [(*g, ds) for g, ds in zip(res, dsinks)]
     return res

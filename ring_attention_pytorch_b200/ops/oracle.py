@@ -47,12 +47,17 @@ def attention_with_positions(
     return_lse: bool = False,
     q_doc: Optional[Tensor] = None,
     k_doc: Optional[Tensor] = None,
+    sinks: Optional[Tensor] = None,
 ):
     """q [b, i, h, d]; k, v [b, j, hk, d]; q_pos [i], k_pos [j] integer global positions.
 
     ``q_doc`` [b, i] / ``k_doc`` [b, j]: document labels, a query sees only keys with its label (on top of every other
     rule).  Labels must be unique per document, e.g. the start column of ``parallel.documents.document_spans``.
     Rows with no visible key produce zeros (and ``lse = +inf``).
+
+    ``sinks`` [h]: learned attention sinks, one logit per query head (not softclamped) that joins every row's softmax
+    denominator with a zero value vector: ``lse = log(exp(sinks[h]) + sum_j exp(s_ij))``, ``out = sum_j exp(s_ij -
+    lse) v_j``.  A row with no visible key gives zeros and ``lse = sinks[h]``.
     """
     b, i, h, d = q.shape
     j = k.shape[1]
@@ -78,12 +83,15 @@ def attention_with_positions(
         visible = visible & (q_doc[:, None, :, None] == k_doc[:, None, None, :])
     neg = torch.finfo(sim.dtype).min
     sim = sim.masked_fill(~visible, neg)
+    if sinks is not None:  # one more column per row: the sink logit, always visible, with a zero value
+        sim = torch.cat((sim, sinks.to(sim.dtype)[None, :, None, None].expand(b, h, i, 1)), dim=-1)
+        visible = torch.cat((visible.expand(b, h, i, j), visible.new_ones(b, h, i, 1)), dim=-1)
     any_vis = visible.any(dim=-1, keepdim=True)
     m = sim.amax(dim=-1, keepdim=True)
     p = (sim - m).exp().masked_fill(~visible, 0.0)
     l = p.sum(dim=-1, keepdim=True)
     attn = torch.where(any_vis, p / l.clamp(min=torch.finfo(sim.dtype).tiny), torch.zeros_like(p))
-    out = torch.einsum("bhij,bjhd->bihd", attn, vx)
+    out = torch.einsum("bhij,bjhd->bihd", attn[..., :j], vx)
     if return_lse:
         lse = torch.where(any_vis, m + l.clamp(min=torch.finfo(sim.dtype).tiny).log(),
                           torch.full_like(m, float("inf"))).squeeze(-1)

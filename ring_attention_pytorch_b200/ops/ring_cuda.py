@@ -64,7 +64,7 @@ from ring_attention_pytorch_b200.parallel.documents import check_document_ids, r
 from ring_attention_pytorch_b200.parallel.layout import make_position_map, ring_hop_owners, ring_query_owners
 from ring_attention_pytorch_b200.parallel.symm import get_workspace
 from ring_attention_pytorch_b200.utils.timing import nvtx_range
-from ring_attention_pytorch_b200.utils.validate import check_attention_inputs, typecheck
+from ring_attention_pytorch_b200.utils.validate import check_attention_inputs, check_sinks, typecheck
 
 # counts launches of our own kernels (bench.py reports it as gpu_launches)
 LAUNCHES = {"count": 0}
@@ -197,6 +197,7 @@ class RingFlashAttentionCUDAFunction(Function):
         layout: Optional[str] = None,
         rotary_freqs: Optional[Tensor] = None,
         document_ids: Optional[Tensor] = None,
+        sinks: Optional[Tensor] = None,
     ):
         assert q.is_cuda and k.is_cuda and v.is_cuda, "ring_flash_attn_cuda needs CUDA tensors"
         ops = _ext.ops()
@@ -252,6 +253,7 @@ class RingFlashAttentionCUDAFunction(Function):
         dev = q.device
         # document masking: the [ring, b, n, 2] interval table, built once here and reused by every launch of the backward
         spans = ring_document_spans(document_ids.to(dev), pm, use_ring) if exists(document_ids) else None
+        sinks32 = sinks.detach().float().contiguous() if exists(sinks) else None
 
         ready = torch.zeros(ring_size, dtype=torch.int32, device=dev)
         peers = [0] * ring_size
@@ -293,23 +295,25 @@ class RingFlashAttentionCUDAFunction(Function):
                     o, lse = fused_attn_fwd_hop(qp, window_slots.slot(s_), owner, ring_size, carry_o, carry_ml, kbits,
                                                 carry_in=s_ > 0, carry_out=s_ + 1 < len(hops), kv_heads=hk, rank=rank,
                                                 pm=pm, causal=causal, window=max_lookback_seq_len, scale=scale,
-                                                softclamp=softclamp, q_pos_offset=q_off, doc_spans=spans)
+                                                softclamp=softclamp, q_pos_offset=q_off, doc_spans=spans,
+                                                sinks=sinks32)
                     window_slots.launched(s_)
                     _count()
                 del carry_o, carry_ml
             else:
                 o, lse = fused_attn_fwd(qp, kv_gather, peers, ready, kbits, kv_heads=hk, rank=rank, pm=pm,
                                         causal=causal, window=max_lookback_seq_len, scale=scale, softclamp=softclamp,
-                                        q_pos_offset=q_off, doc_spans=spans)
+                                        q_pos_offset=q_off, doc_spans=spans, sinks=sinks32)
                 _count()
 
         ctx.cfg = (causal, max_lookback_seq_len, ring_size, rank, layout, softclamp, scale, q_off, use_ring, d, d_pad,
-                   orig_dtype, hk, fused_k_rotary)
+                   orig_dtype, hk, fused_k_rotary, sinks.dtype if exists(sinks) else None)
         # single rank: the packed K/V is exactly what the backward needs; ring: keep the (small) inputs, re-pack later
         none = torch.empty(0, device=dev)
         ctx.save_for_backward(qp, kp if use_ring else none, vp if use_ring else none, o, lse,
                               none if use_ring else kv_gather, kbits if kbits is not None else none,
-                              ang if ang is not None else none, spans if spans is not None else none)
+                              ang if ang is not None else none, spans if spans is not None else none,
+                              sinks32 if sinks32 is not None else none)
         out = o[..., :d]
         return out.to(orig_dtype) if orig_dtype != dt else out
 
@@ -317,11 +321,12 @@ class RingFlashAttentionCUDAFunction(Function):
     def backward(ctx, do: Tensor):
         ops = _ext.ops()
         (causal, window, ring_size, rank, layout, softclamp, scale, q_off, use_ring, d, d_pad, orig_dtype,
-         hk, fused_k_rotary) = ctx.cfg
-        qp, kp, vp, o, lse, kv_saved, kbits, ang, spans = ctx.saved_tensors
+         hk, fused_k_rotary, sinks_dtype) = ctx.cfg
+        qp, kp, vp, o, lse, kv_saved, kbits, ang, spans, sinks32 = ctx.saved_tensors
         kbits = kbits if kbits.numel() > 0 else None
         ang = ang if ang.numel() > 0 else None
         spans = spans if spans.numel() > 0 else None
+        sinks32 = sinks32 if sinks_dtype is not None else None
         dt = qp.dtype
         b, n_q, h, _ = qp.shape
         dev = qp.device
@@ -329,6 +334,8 @@ class RingFlashAttentionCUDAFunction(Function):
         n_k = kp.shape[1] if use_ring else kv_saved.shape[3]
         pm = make_position_map(layout, ring_size, max(n_q, n_k))
         hop_owner = ring_hop_owners(pm, rank, causal, window)
+        # the sink gradient of this rank's rows, reduced by bwd_prep from the lse and delta it writes
+        dsinks = torch.empty(h, dtype=torch.float32, device=dev) if sinks32 is not None else None
 
         ws = None
         kv_own_ptrs, kv_bytes = None, 0
@@ -370,7 +377,7 @@ class RingFlashAttentionCUDAFunction(Function):
             with nvtx_range("rab.bwd.prep"):
                 qdo = alloc_qdo_buffer(1, b, h, n_q, d_pad, dt, dev)
                 stat = alloc_stat_buffer(1, b, h, n_q, dev)
-                ops.bwd_prep(qp, o, dop, lse, qdo, stat, 0)
+                ops.bwd_prep(qp, o, dop, lse, qdo, stat, 0, sinks32, dsinks)
                 dq_acc = torch.zeros(b * h, stat.shape[-1], d_pad, dtype=torch.float32, device=dev)
                 _count(2)
             ready, ready_target, side_done, acc, acc_ptrs, nk_pad = None, 0, None, None, (), 0
@@ -422,7 +429,7 @@ class RingFlashAttentionCUDAFunction(Function):
             # ---------------- two-kernel backward (csrc/attn_bwd_sm90.cu) ----------------
             qdo_gather = alloc_qdo_buffer(ring_size, b, h, n_q, d_pad, dt, dev)
             stat_gather = alloc_stat_buffer(ring_size, b, h, n_q, dev)
-            ops.bwd_prep(qp, o, dop, lse, qdo_gather, stat_gather, rank)
+            ops.bwd_prep(qp, o, dop, lse, qdo_gather, stat_gather, rank, sinks32, dsinks)
             _count()
             ready_kv, gather_done = None, None
             if use_ring:
@@ -463,7 +470,9 @@ class RingFlashAttentionCUDAFunction(Function):
             dq, dk = dq_in, dk_in
         if orig_dtype != dt:
             dq, dk, dv = dq.to(orig_dtype), dk.to(orig_dtype), dv.to(orig_dtype)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None, None
+        if dsinks is not None:
+            dsinks = dsinks.to(sinks_dtype)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None, None, dsinks
 
 
 ring_flash_attn_cuda_ = RingFlashAttentionCUDAFunction.apply
@@ -487,6 +496,7 @@ def ring_flash_attn_cuda(
     layout: Optional[str] = None,
     rotary_freqs: Optional[Tensor] = None,
     document_ids: Optional[Tensor] = None,
+    sinks: Optional[Tensor] = None,
 ) -> Tensor:
     """q [b, n, h, d]; k, v [b, n, hk, d] (this rank's shard when ``ring_reduce_col``).  ``bucket_size`` is
     accepted for signature parity; tiling is fixed by the kernel (128 x 128).  ``rotary_freqs`` ([n, d] or [n, d/2]
@@ -497,9 +507,14 @@ def ring_flash_attn_cuda(
     sequences.  A document is a maximal run of equal ids in global position order (two separate runs sharing an id are
     two documents); a query sees only keys of its own document, on top of ``causal``, the look-back window and
     ``mask``.  Unlike ``mask`` it is kept under ``causal=True``.  Self-attention only.  Tiles that no document
-    crosses are skipped without being loaded, so packed causal training does only the visible work."""
+    crosses are skipped without being loaded, so packed causal training does only the visible work.
+
+    ``sinks`` (floating ``[h]``): learned attention sinks, see :func:`ring_flash_attn`.  The forward kernel starts each
+    row's softmax state from the sink; the backward returns its gradient (this rank's rows, in ``sinks``' dtype),
+    reduced in a fixed order, so the two-kernel backward stays deterministic."""
     check_attention_inputs(q, k, v, mask, name="ring_flash_attn_cuda", max_head_dim=128)
     check_document_ids(document_ids, q, k)
+    check_sinks(sinks, q.shape[2], q.device, name="ring_flash_attn_cuda")
     return ring_flash_attn_cuda_(q, k, v, mask, causal, bucket_size, ring_reduce_col, striped_ring_attn,
                                  max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value, layout,
-                                 rotary_freqs, document_ids)
+                                 rotary_freqs, document_ids, sinks)

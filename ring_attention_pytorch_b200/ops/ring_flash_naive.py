@@ -11,7 +11,8 @@ maps instead of bucket bookkeeping:
   by the exact remaining distance (the reference sends it every iteration and mis-unpacks the result –
   reference ring_flash_attention.py:377-385, SURVEY defect D1/D2/D3);
 * fully masked rows give 0 output (never NaN);
-* document masking for packed sequences (``document_ids``, see :mod:`ring_attention_pytorch_b200.parallel.documents`).
+* document masking for packed sequences (``document_ids``, see :mod:`ring_attention_pytorch_b200.parallel.documents`);
+* learned attention sinks (``sinks``): folded into each row's softmax state once, after the last hop.
 """
 from __future__ import annotations
 
@@ -25,7 +26,7 @@ from ring_attention_pytorch_b200.parallel.distributed import default, exists, ge
 from ring_attention_pytorch_b200.parallel.documents import check_document_ids, document_mask, ring_document_spans
 from ring_attention_pytorch_b200.parallel.layout import PositionMap, make_position_map, ring_hop_owners
 from ring_attention_pytorch_b200.parallel.ring import all_ring_pass, null_ring_pass, ring_pass
-from ring_attention_pytorch_b200.utils.validate import check_attention_inputs, typecheck
+from ring_attention_pytorch_b200.utils.validate import check_attention_inputs, check_sinks, typecheck
 
 EPSILON = 1e-10
 
@@ -80,6 +81,7 @@ class RingFlashAttentionFunction(Function):
         softclamp_value: float = 50.0,
         layout: Optional[str] = None,
         document_ids: Optional[Tensor] = None,
+        sinks: Optional[Tensor] = None,
     ):
         check_document_ids(document_ids, q, k)
         ring_size = default(ring_size, get_world_size())
@@ -150,6 +152,15 @@ class RingFlashAttentionFunction(Function):
                 o[:, s:e] = o[:, s:e] * corr + torch.einsum("bighj,bjhd->bighd", p, vc)
                 row_max[:, s:e] = new_max
 
+        if exists(sinks):
+            # the sink logit joins every row's denominator once, with a zero value vector
+            sink = sinks.float().view(1, 1, qf.shape[2], hk, 1)
+            new_max = torch.maximum(row_max, sink)
+            corr = (row_max - new_max).exp()
+            row_sum = row_sum * corr + (sink - new_max).exp()
+            o = o * corr
+            row_max = new_max
+
         has_any = row_sum > 0
         o = torch.where(has_any, o / row_sum.clamp(min=EPSILON), torch.zeros_like(o))
         lse = torch.where(has_any, row_sum.clamp(min=EPSILON).log() + row_max, torch.full_like(row_max, float("inf")))
@@ -157,7 +168,7 @@ class RingFlashAttentionFunction(Function):
 
         ctx.args = (causal, scale, mask, bucket, ring_reduce_col, ring_size, max_iters, max_lookback_seq_len,
                     softclamp_qk_sim, softclamp_value, layout, cross_attn, rank, q_spans)
-        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.save_for_backward(q, k, v, out, lse, sinks if exists(sinks) else torch.empty(0))
         return out
 
     @staticmethod
@@ -165,7 +176,7 @@ class RingFlashAttentionFunction(Function):
     def backward(ctx, do: Tensor):
         (causal, scale, mask, bucket, ring_reduce_col, ring_size, max_iters, window, softclamp_qk_sim,
          softclamp_value, layout, cross_attn, rank, q_spans) = ctx.args
-        q, k, v, o, lse = ctx.saved_tensors
+        q, k, v, o, lse, sinks = ctx.saved_tensors
         b, n, h, d = q.shape
         n_k, hk = k.shape[1], k.shape[2]
         pm = make_position_map(layout, ring_size, n_k)
@@ -177,6 +188,10 @@ class RingFlashAttentionFunction(Function):
         of = _group_q(o.float(), hk)
         delta = (dof * of).sum(dim=-1, keepdim=True)
         dq = torch.zeros_like(qf)
+        dsinks = None
+        if sinks.numel() > 0:  # d lse / d sink = exp(sink - lse); this rank's rows only
+            sink = sinks.float().view(1, 1, qf.shape[2], hk, 1)
+            dsinks = -((sink - lse).exp() * delta).sum(dim=(0, 1)).reshape(h).to(sinks.dtype)
 
         # (k, v, dk, dv) ride the ring together in fp32 (reference carries them in the activation dtype)
         packet = torch.stack((k.float(), v.float(), torch.zeros_like(k, dtype=torch.float32),
@@ -235,7 +250,8 @@ class RingFlashAttentionFunction(Function):
             dk, dv = last_packet[2], last_packet[3]
 
         dq = dq.reshape(b, n, h, d).to(q.dtype)
-        return dq, dk.to(k.dtype), dv.to(v.dtype), None, None, None, None, None, None, None, None, None, None, None
+        return (dq, dk.to(k.dtype), dv.to(v.dtype), None, None, None, None, None, None, None, None, None, None, None,
+                dsinks)
 
 
 ring_flash_attn_ = RingFlashAttentionFunction.apply
@@ -257,13 +273,20 @@ def ring_flash_attn(
     softclamp_value: float = 50.0,
     layout: Optional[str] = None,
     document_ids: Optional[Tensor] = None,
+    sinks: Optional[Tensor] = None,
 ) -> Tensor:
     """Reference-compatible signature (ring_flash_attention.py:391-406) + ``layout`` ('plain'|'striped'|'zigzag').
 
     ``document_ids`` (integer ``[b, n]``, sharded and laid out like ``q``): document masking for packed sequences.  A
     document is a maximal run of equal ids in global position order (two separate runs sharing an id are two
     documents); a query sees only keys of its own document, on top of ``causal``, the look-back window and ``mask``.
-    Unlike ``mask`` it is kept under ``causal=True``.  Self-attention only."""
+    Unlike ``mask`` it is kept under ``causal=True``.  Self-attention only.
+
+    ``sinks`` (floating ``[h]``): learned attention sinks, one logit per query head (not softclamped) that joins every
+    row's softmax denominator once, with a zero value vector.  A row that sees no key gives 0.  Its gradient is this
+    rank's partial sum over its own rows, like every other parameter's."""
     check_attention_inputs(q, k, v, mask, name="ring_flash_attn")
+    check_sinks(sinks, q.shape[2], q.device, name="ring_flash_attn")
     return ring_flash_attn_(q, k, v, mask, causal, bucket_size, ring_reduce_col, striped_ring_attn,
-                            max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value, layout, document_ids)
+                            max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value, layout, document_ids,
+                            sinks)

@@ -83,7 +83,7 @@ def dequantized_ring_flash_attn(q, k, v, q_descale, k_descale, v_descale, *args,
 @torch.no_grad()
 def _ring_flash_attn_fp8_cuda(q, k, v, q_descale, k_descale, v_descale, mask, causal, ring_reduce_col,
                               striped_ring_attn, max_lookback_seq_len, ring_size, softclamp_qk_sim, softclamp_value,
-                              layout, document_ids) -> Tensor:
+                              layout, document_ids, sinks) -> Tensor:
     from ring_attention_pytorch_b200.ops import _ext, ring_cuda
     from ring_attention_pytorch_b200.ops.fused import (alloc_fwd_carry, alloc_kv_buffer_fp8, fused_attn_fwd_fp8,
                                                        fused_attn_fwd_hop_fp8, pack_key_mask_bits, pack_kv_fp8, pad128)
@@ -115,6 +115,7 @@ def _ring_flash_attn_fp8_cuda(q, k, v, q_descale, k_descale, v_descale, mask, ca
     q_off = (n_k - n_q) if (cross_attn and causal) else 0
     dev = q.device
     spans = ring_document_spans(document_ids.to(dev), pm, use_ring) if exists(document_ids) else None
+    sinks = sinks.float().contiguous() if exists(sinks) else None
 
     # an fp8 slot [2, b*hk, n_pad, 128] has the bytes of a bf16 slot of n_pad / 2 keys: the workspaces, the copy-engine
     # window and the fetcher warps only move bytes
@@ -162,13 +163,13 @@ def _ring_flash_attn_fp8_cuda(q, k, v, q_descale, k_descale, v_descale, mask, ca
                                               carry_ml, kbits, carry_in=s_ > 0, carry_out=s_ + 1 < len(hops),
                                               kv_heads=hk, rank=rank, pm=pm, causal=causal,
                                               window=max_lookback_seq_len, scale=scale, softclamp=softclamp,
-                                              q_pos_offset=q_off, doc_spans=spans)
+                                              q_pos_offset=q_off, doc_spans=spans, sinks=sinks)
                 window_slots.launched(s_)
                 ring_cuda._count()
         else:
             o, _ = fused_attn_fwd_fp8(q, kv_gather, n_k, descales, peers, ready, kbits, kv_heads=hk, rank=rank, pm=pm,
                                       causal=causal, window=max_lookback_seq_len, scale=scale, softclamp=softclamp,
-                                      q_pos_offset=q_off, doc_spans=spans)
+                                      q_pos_offset=q_off, doc_spans=spans, sinks=sinks)
             ring_cuda._count()
     return o
 
@@ -194,20 +195,22 @@ def ring_flash_attn_fp8(
     layout: Optional[str] = None,
     document_ids: Optional[Tensor] = None,
     rotary_freqs: Optional[Tensor] = None,
+    sinks: Optional[Tensor] = None,
 ) -> Tensor:
     """Ring attention forward on e4m3 inputs (see the module docstring for the exact semantics).
 
     q ``[b, n, h, 128]``, k / v ``[b, n, hk, 128]`` ``float8_e4m3fn``, sharded and laid out as for
     :func:`ring_flash_attn_cuda`; ``q_descale`` fp32 ``[b, h]``, ``k_descale`` / ``v_descale`` fp32 ``[b, hk]`` (one
     element broadcasts).  Every other argument has the meaning it has there.  Returns bf16 ``[b, n, h, 128]``.
-    ``rotary_freqs`` is refused: rotate q and k before quantising them."""
+    ``rotary_freqs`` is refused: rotate q and k before quantising them.  ``sinks`` (floating ``[h]``, not requiring
+    grad): learned attention sinks in the logits' natural-log units, as in :func:`ring_flash_attn`."""
     check_fp8_attention_inputs(q, k, v, q_descale, k_descale, v_descale, mask, name="ring_flash_attn_fp8",
-                               rotary_freqs=rotary_freqs)
+                               rotary_freqs=rotary_freqs, sinks=sinks)
     check_document_ids(document_ids, q, k)
     kwargs = dict(mask=mask, causal=causal, bucket_size=bucket_size, ring_reduce_col=ring_reduce_col,
                   striped_ring_attn=striped_ring_attn, max_lookback_seq_len=max_lookback_seq_len, ring_size=ring_size,
                   softclamp_qk_sim=softclamp_qk_sim, softclamp_value=softclamp_value, layout=layout,
-                  document_ids=document_ids)
+                  document_ids=document_ids, sinks=sinks)
     if not q.is_cuda:
         return dequantized_ring_flash_attn(q, k, v, q_descale, k_descale, v_descale, **kwargs)
     if q.shape[3] != 128:

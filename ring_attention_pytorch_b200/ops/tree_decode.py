@@ -22,7 +22,7 @@ import torch.distributed as dist
 from torch import Tensor
 
 from ring_attention_pytorch_b200.parallel.distributed import default, exists, get_rank, get_world_size, is_distributed
-from ring_attention_pytorch_b200.utils.validate import typecheck
+from ring_attention_pytorch_b200.utils.validate import check_sinks, typecheck
 
 
 def _local_attention(q: Tensor, k: Tensor, v: Tensor):
@@ -49,6 +49,7 @@ def tree_attn_decode(
     shard_kv_seq: bool = True,
     use_triton: Optional[bool] = None,
     dim_v: Optional[int] = None,
+    sinks: Optional[Tensor] = None,
 ) -> Tensor:
     """Returns ``[b, h, 1, dv]`` in ``q.dtype``.
 
@@ -56,10 +57,14 @@ def tree_attn_decode(
     (ranks beyond the number of chunks contribute nothing).  ``shard_kv_seq=False``: K/V are already this
     rank's shard (``None`` for an empty shard).  ``use_triton`` is kept for signature parity and selects the
     sm_90a kernel (default: on CUDA inputs).
+
+    ``sinks`` (floating ``[h]``): learned attention sinks, one logit per query head with a zero value vector.  The
+    softmax runs over the keys of every rank and the sink, which is added once, in the cross-rank merge.
     """
     assert not (exists(k) ^ exists(v)), "keys and values are either both None, or both present"
     dtype = q.dtype
     b, h = q.shape[:2]
+    check_sinks(sinks, h, q.device, name="tree_attn_decode")
     if exists(v):
         dim_v = v.shape[-1]
 
@@ -76,7 +81,7 @@ def tree_attn_decode(
     if use_kernel:
         from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda
 
-        return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps).to(dtype)
+        return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps, sinks=sinks).to(dtype)
 
     if exists(k) and k.shape[-2] > 0:
         local_out, lse = _local_attention(q, k, v)
@@ -84,13 +89,20 @@ def tree_attn_decode(
         local_out = q.new_zeros((b, h, 1, dim_v), dtype=torch.float32)
         lse = torch.full((b, h, 1, 1), -torch.finfo(torch.float32).max, device=q.device, dtype=torch.float32)
 
-    if not is_distributed():
+    if not is_distributed() and not exists(sinks):
         return local_out.to(dtype)
 
     max_lse = lse.clone()
-    dist.all_reduce(max_lse, dist.ReduceOp.MAX)
+    if is_distributed():
+        dist.all_reduce(max_lse, dist.ReduceOp.MAX)
+    if exists(sinks):
+        sink = sinks.float().view(1, h, 1, 1)
+        max_lse = torch.maximum(max_lse, sink)
     den = (lse - max_lse).exp()
     packed = torch.cat((local_out * den, den), dim=-1)  # numerator | denominator in one collective
-    dist.all_reduce(packed)
+    if is_distributed():
+        dist.all_reduce(packed)
     num, den = packed[..., :-1], packed[..., -1:]
+    if exists(sinks):  # the sink joins the merged denominator once, after the reduction
+        den = den + (sink - max_lse).exp()
     return (num / den.clamp(min=eps)).to(dtype)

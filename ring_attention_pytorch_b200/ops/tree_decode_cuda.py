@@ -147,6 +147,7 @@ def tree_decode_cuda(
     v_scale: Optional[Tensor] = None,
     scale_block_keys: int = 0,
     out: Optional[Tensor] = None,
+    sinks: Optional[Tensor] = None,
 ) -> Tensor:
     """q [b, h, 1, d] (bf16 / fp16 / fp32); k, v [b, hk, n, d] this rank's shard (bf16 / fp16 / float8_e4m3fn) or None.
     k / v may be the filled prefix ``cache[:, :, :n]`` of a larger ``[b, hk, capacity, d]`` buffer: the tensor-core kernel
@@ -155,7 +156,8 @@ def tree_decode_cuda(
     ``k_scale`` / ``v_scale``: optional fp32 dequantisation scales for the fp8 path, either per (batch, kv head)
     (``numel == b*hk``) or block-scaled ``[b*hk, n_blocks]`` with one scale per ``scale_block_keys`` keys
     (a multiple of 64).  ``out`` ([b, h, 1, d]) may be passed to make the call allocation free (CUDA graphs).
-    Returns [b, h, 1, d] in q's dtype.
+    ``sinks`` (``[h]``, fp32 contiguous for an allocation-free call): learned attention sinks, added once, in the
+    kernel's cross-rank merge.  Returns [b, h, 1, d] in q's dtype.
     """
     ops = _ext.ops()
     b, h, _, d = q.shape
@@ -192,10 +194,12 @@ def tree_decode_cuda(
     if out is None:
         out_dtype = q.dtype if q.dtype in (torch.bfloat16, torch.float16) else torch.float32
         out = torch.empty(b, h, 1, d, dtype=out_dtype, device=dev)
+    if sinks is not None:
+        sinks = sinks.float().contiguous()
     units = groups * splits if n > 0 else 0
     grid = max(1, min(resident, max(units, (b * h + 3) // 4)))
     ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
                     buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out.view(b, h, d), hk,
-                    splits, d ** -0.5, scale_block_keys, eps, grid, use_tc)
+                    splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks)
     LAUNCHES["count"] += 1
     return out

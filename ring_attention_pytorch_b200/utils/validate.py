@@ -58,11 +58,25 @@ def check_attention_inputs(q: Tensor, k: Tensor, v: Tensor, mask: Optional[Tenso
                              f"{mask.dtype} {tuple(mask.shape)}")
 
 
+def check_sinks(sinks: Optional[Tensor], heads: int, device, *, name: str = "attention") -> None:
+    """Learned attention sinks: a floating ``[heads]`` tensor (one logit per query head) on the inputs' device."""
+    if sinks is None:
+        return
+    if not torch.is_tensor(sinks) or sinks.dim() != 1 or sinks.shape[0] != heads:
+        raise ValueError(f"{name}: sinks must be a 1-D tensor of one logit per query head [{heads}], got "
+                         f"{tuple(sinks.shape) if torch.is_tensor(sinks) else type(sinks)}")
+    if not sinks.is_floating_point():
+        raise ValueError(f"{name}: sinks must be a floating tensor, got {sinks.dtype}")
+    if sinks.device != torch.device(device):
+        raise ValueError(f"{name}: sinks must live on {device}, got {sinks.device}")
+
+
 def check_fp8_attention_inputs(q: Tensor, k: Tensor, v: Tensor, q_descale, k_descale, v_descale,
                                mask: Optional[Tensor] = None, *, name: str = "attention",
-                               rotary_freqs: Optional[Tensor] = None) -> None:
+                               rotary_freqs: Optional[Tensor] = None, sinks: Optional[Tensor] = None) -> None:
     """Inputs of the fp8 forward: e4m3 q / k / v with the shapes of :func:`check_attention_inputs`, fp32 descales
-    ``[b, h]`` (q) and ``[b, hk]`` (k, v) or one element each, nothing that requires grad, no rotary angles."""
+    ``[b, h]`` (q) and ``[b, hk]`` (k, v) or one element each, sinks as :func:`check_sinks`, nothing that requires
+    grad, no rotary angles."""
     check_attention_inputs(q, k, v, mask, name=name)
     for nm, t in (("q", q), ("k", k), ("v", v)):
         if t.dtype != torch.float8_e4m3fn:
@@ -76,7 +90,8 @@ def check_fp8_attention_inputs(q: Tensor, k: Tensor, v: Tensor, q_descale, k_des
                              f"{tuple(t.shape)}")
         if t.device != q.device:
             raise ValueError(f"{name}: {nm} must live on {q.device}, got {t.device}")
-    if any(t.requires_grad for t in (q, k, v, q_descale, k_descale, v_descale)):
+    check_sinks(sinks, h, q.device, name=name)
+    if any(t is not None and t.requires_grad for t in (q, k, v, q_descale, k_descale, v_descale, sinks)):
         raise ValueError(f"{name}: the fp8 attention is forward only; an input requires grad")
     if rotary_freqs is not None:
         raise ValueError(f"{name}: rotary_freqs is not accepted; rotate q and k first, then quantise them")

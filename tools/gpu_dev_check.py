@@ -74,9 +74,11 @@ def _doc_labels(doc_ids, layout, n):
     return [spans[r, ..., 0] for r in range(len(doc_ids))]
 
 
-def _ref_ring(qs, ks, vs, layout, causal, window, softclamp, key_masks, doc_ids=None, dos=None, dtype=None):
+def _ref_ring(qs, ks, vs, layout, causal, window, softclamp, key_masks, doc_ids=None, dos=None, dtype=None,
+              sinks=None):
     """The oracle over the whole emulated ring: per-rank (outs, lses), and with ``dos`` also per-rank (dq, dk, dv)
-    through autograd.  ``dtype`` (default fp32) is the precision the oracle computes in."""
+    through autograd.  ``dtype`` (default fp32) is the precision the oracle computes in.  ``sinks`` ([h] attention
+    sinks): with ``dos`` every rank's tuple gains that rank's own sink gradient (its rows only), as the kernels give."""
     import torch
     from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
     from ring_attention_pytorch_b200.parallel.layout import make_position_map
@@ -93,22 +95,29 @@ def _ref_ring(qs, ks, vs, layout, causal, window, softclamp, key_masks, doc_ids=
     k_pos = torch.cat([pm.positions(r, qs[0].device) for r in range(world)])
     km = None if key_masks is None else torch.cat(list(key_masks), 1)
     labels = _doc_labels(doc_ids, layout, n) if doc_ids is not None else None
-    outs, lses = [], []
+    sf = None if sinks is None else sinks.detach().to(dtype).clone().requires_grad_(grad)
+    outs, lses, dsinks = [], [], []
     loss = 0.0
     with torch.enable_grad():
         for r in range(world):
             o, lse = attention_with_positions(qf[r], k_all, v_all, pm.positions(r, qs[0].device), k_pos,
                                               causal=causal, window=window, key_mask=km, softclamp_value=softclamp,
                                               return_lse=True, q_doc=None if labels is None else labels[r],
-                                              k_doc=None if labels is None else torch.cat(labels, 1))
+                                              k_doc=None if labels is None else torch.cat(labels, 1), sinks=sf)
             outs.append(o.detach())
             lses.append(lse.detach())
             if grad:
-                loss = loss + (o * dos[r].to(dtype)).sum()
+                loss_r = (o * dos[r].to(dtype)).sum()
+                if sf is not None:
+                    dsinks.append(torch.autograd.grad(loss_r, sf, retain_graph=True)[0])
+                loss = loss + loss_r
         if not grad:
             return outs, lses
         loss.backward()
-    return outs, lses, [(qf[r].grad, kf[r].grad, vf[r].grad) for r in range(world)]
+    grads = [(qf[r].grad, kf[r].grad, vf[r].grad) for r in range(world)]
+    if sf is not None:
+        grads = [(*g, ds) for g, ds in zip(grads, dsinks)]
+    return outs, lses, grads
 
 
 # ----------------------------------------------------------------------------------------------
@@ -325,6 +334,35 @@ def make_case_inputs(regime, world, b, n, h, hk, d, dt, layout="plain", causal=F
     return shards(q), shards(k), shards(v), shards(do)
 
 
+def make_sinks(kind, qs, ks, softclamp=0.0):
+    """fp32 ``[h]`` attention sinks of a case (``sinks=`` option), placed against the case's own logits (natural log,
+    after scale and softclamp):
+
+    below : 10 nats below the head's median row maximum
+    near  : at the head's median row maximum
+    above : 10 nats above every logit of the head
+    mix   : the heads cycle through below, near and above
+    """
+    import torch
+    from ring_attention_pytorch_b200.ops.oracle import expand_kv_heads
+
+    h, d = qs[0].shape[2], qs[0].shape[3]
+    k_all = expand_kv_heads(torch.cat([k.float() for k in ks], 1), h)
+    row_max, top = [], torch.full((h,), -float("inf"), device=qs[0].device)
+    for q in qs:
+        s = torch.einsum("bihd,bjhd->bhij", q.float(), k_all) * d ** -0.5
+        if softclamp:
+            s = (s / softclamp).tanh() * softclamp
+        m = s.amax(-1)
+        row_max.append(m.transpose(0, 1).reshape(h, -1))
+        top = torch.maximum(top, m.amax(dim=(0, 2)))
+    med = torch.cat(row_max, 1).median(1).values
+    choice = {"below": med - 10.0, "near": med, "above": top + 10.0}
+    if kind == "mix":
+        return torch.stack([choice[("below", "near", "above")[i % 3]][i] for i in range(h)]).contiguous()
+    return choice[kind].contiguous()
+
+
 def _case_docs(docs, b, n, world, layout, kmask, seed):
     """(per-rank document ids, per-rank key masks) of a case."""
     import torch
@@ -358,53 +396,82 @@ def _case_inputs(regime, world, b, n, h, hk, d, dtype, layout, causal, window, s
     return qs, ks, vs, dos, doc_ids, kms, info
 
 
+def _empty_rows(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, rlses, sk):
+    """Per-rank [b, h, n] masks of the rows that see no key (with sinks their lse is finite: ask a sink-free oracle)."""
+    import torch
+
+    if sk is not None:
+        qs, ks, vs = ([t.detach() for t in ts] for ts in (qs, ks, vs))
+        rlses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids)[1]
+    return [torch.isinf(l) for l in rlses]
+
+
 def case_fwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=False, window=None, softclamp=0.0,
-             kmask=False, dtype="bf16", seed=0, hopwise=False, docs=None, regime=None):
+             kmask=False, dtype="bf16", seed=0, hopwise=False, docs=None, regime=None, sinks=None):
     import torch
     from ring_attention_pytorch_b200.ops.fused import emulate_ring_forward
 
     hk = hk or h
     qs, ks, vs, _, doc_ids, kms, info = _case_inputs(regime, world, b, n, h, hk, d, dtype, layout, causal, window,
                                                      softclamp, kmask, docs, seed, False)
+    sk = None if sinks is None else make_sinks(sinks, qs, ks, softclamp)
     outs, lses = emulate_ring_forward(qs, ks, vs, layout=layout, causal=causal, window=window, softclamp=softclamp,
-                                      key_masks=kms, hopwise=hopwise, document_ids=doc_ids)
+                                      key_masks=kms, hopwise=hopwise, document_ids=doc_ids, sinks=sk)
     torch.cuda.synchronize()
-    routs, rlses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids)
-    louts, llses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, dtype=qs[0].dtype)
+    routs, rlses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, sinks=sk)
+    louts, llses = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, dtype=qs[0].dtype, sinks=sk)
     res = {"out": noise_bound(outs, routs, louts, CAP_OUT), "lse": noise_bound(lses, rlses, llses, CAP_LSE), **info}
-    # rows that see no key: exactly zero output (the rule above only bounds them by its epsilon)
-    res["empty_rows_exact"] = all(bool((o.float()[torch.isinf(l).transpose(1, 2)] == 0).all())
-                                  for o, l in zip(outs, rlses))
+    # rows that see no key: exactly zero output (the rule above only bounds them by its epsilon); with sinks their
+    # lse is the sink's
+    empty = _empty_rows(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, rlses, sk)
+    res["empty_rows_exact"] = all(bool((o.float()[e.transpose(1, 2)] == 0).all()) for o, e in zip(outs, empty))
+    if sk is not None:
+        res["empty_rows_lse_is_sink"] = all(
+            bool(((l - sk[None, :, None]).abs()[e] <= 1e-5 * (1 + sk.abs().max())).all()) for l, e in zip(lses, empty))
+        res["empty_rows_exact"] = res["empty_rows_exact"] and res["empty_rows_lse_is_sink"]
     res["ok"] = res["out"]["ok"] and res["lse"]["ok"] and res["empty_rows_exact"]
     return res
 
 
 def case_bwd(world=1, b=1, n=256, h=2, hk=None, d=128, layout="plain", causal=False, window=None, softclamp=0.0,
-             kmask=False, dtype="bf16", seed=0, fused=None, hopwise=False, docs=None, regime=None):
+             kmask=False, dtype="bf16", seed=0, fused=None, hopwise=False, docs=None, regime=None, sinks=None):
+    """With ``sinks`` the result also holds ``dsinks`` (every rank's sink gradient against the oracle's) and
+    ``dsinks_deterministic`` (a second backward gives bitwise the same sink gradients)."""
     import torch
     from ring_attention_pytorch_b200.ops.fused import emulate_ring_backward, emulate_ring_forward
 
     hk = hk or h
     qs, ks, vs, dos, doc_ids, kms, info = _case_inputs(regime, world, b, n, h, hk, d, dtype, layout, causal, window,
                                                        softclamp, kmask, docs, seed, True)
+    sk = None if sinks is None else make_sinks(sinks, qs, ks, softclamp)
     outs, lses = emulate_ring_forward(qs, ks, vs, layout=layout, causal=causal, window=window, softclamp=softclamp,
-                                      key_masks=kms, hopwise=hopwise, document_ids=doc_ids)
-    grads = emulate_ring_backward(qs, ks, vs, outs, lses, dos, layout=layout, causal=causal, window=window,
-                                  softclamp=softclamp, key_masks=kms, fused=fused, hopwise=hopwise,
-                                  document_ids=doc_ids)
+                                      key_masks=kms, hopwise=hopwise, document_ids=doc_ids, sinks=sk)
+
+    def backward():
+        return emulate_ring_backward(qs, ks, vs, outs, lses, dos, layout=layout, causal=causal, window=window,
+                                     softclamp=softclamp, key_masks=kms, fused=fused, hopwise=hopwise,
+                                     document_ids=doc_ids, sinks=sk)
+
+    grads = backward()
+    again = backward() if sk is not None else None
     torch.cuda.synchronize()
-    _, rlses, ref = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, dos=dos)
-    _, _, lowp = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, dos=dos, dtype=qs[0].dtype)
+    _, rlses, ref = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, dos=dos, sinks=sk)
+    _, _, lowp = _ref_ring(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, dos=dos, dtype=qs[0].dtype,
+                           sinks=sk)
+    names = ("dq", "dk", "dv") if sk is None else ("dq", "dk", "dv", "dsinks")
     res = {name: noise_bound([g[i] for g in grads], [x[i] for x in ref], [x[i] for x in lowp],
                              CAP_GRAD_REL * max(x[i].abs().max().item() for x in ref))
-           for i, name in enumerate(("dq", "dk", "dv"))}
+           for i, name in enumerate(names)}
     res.update(info)
+    if sk is not None:
+        res["dsinks_deterministic"] = all(bool(torch.equal(g[3], a[3])) for g, a in zip(grads, again))
     # exact zeros: dq of rows that see no key, dk / dv of masked keys (no query sees them)
-    exact = all(bool((g[0].float()[torch.isinf(l).transpose(1, 2)] == 0).all()) for g, l in zip(grads, rlses))
+    empty = _empty_rows(qs, ks, vs, layout, causal, window, softclamp, kms, doc_ids, rlses, sk)
+    exact = all(bool((g[0].float()[e.transpose(1, 2)] == 0).all()) for g, e in zip(grads, empty))
     if kms is not None:
         exact = exact and all(bool((g[i].float()[~m] == 0).all()) for g, m in zip(grads, kms) for i in (1, 2))
     res["empty_rows_exact"] = exact
-    ok = all(res[k2]["ok"] for k2 in ("dq", "dk", "dv")) and exact
+    ok = all(res[k2]["ok"] for k2 in names) and exact and res.get("dsinks_deterministic", True)
     res["ok"] = ok
     if not ok:
         # localise: per rank / tensor / head / 128-row tile error (nan -> 999)
