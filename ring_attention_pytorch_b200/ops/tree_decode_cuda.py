@@ -37,6 +37,25 @@ def _choose_splits(n: int, groups: int, resident_ctas: int) -> int:
     return max(1, min(want, (n + 255) // 256))
 
 
+@dataclass(frozen=True)
+class DecodePlan:
+    tensor_core: bool  # which kernel runs: the wgmma kernel or the CUDA-core kernel
+    groups: int        # (batch, kv head, head chunk) groups; work units = groups * splits
+    resident: int      # co-resident CTAs of the kernel on this device (the persistent grid's size limit)
+    splits: int        # key splits per group
+
+
+def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int) -> DecodePlan:
+    """The kernel and the work split a decode call of these sizes gets (``kv_kind``: 0 bf16, 1 fp16, 2 fp8 cache)."""
+    tc = CONFIG["tensor_core"]
+    use_tc = tc in ("auto", True, "on") and d == 128 and n >= 1
+    g = h // hk
+    gm = (8 if g <= 8 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: MMA N)
+    groups = b * hk * ((g + gm - 1) // gm)
+    resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc))
+    return DecodePlan(use_tc, groups, resident, _choose_splits(n, groups, resident))
+
+
 @dataclass
 class _Buffers:
     rows: int
@@ -177,14 +196,10 @@ def tree_decode_cuda(
         k = v = None
     g = h // hk
     kv_kind = 0 if k is None or k.dtype == torch.bfloat16 else (1 if k.dtype == torch.float16 else 2)
-    tc = CONFIG["tensor_core"]
-    use_tc = tc in ("auto", True, "on") and d == 128 and n >= 1
+    plan = decode_plan(b, h, hk, n, d, kv_kind)
+    use_tc, groups, resident, splits = plan.tensor_core, plan.groups, plan.resident, plan.splits
     if k is not None and not (use_tc and _is_cache_prefix(k) and v.stride() == k.stride()):
         k, v = k.contiguous(), v.contiguous()  # no-op for dense inputs
-    gm = (8 if g <= 8 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: MMA N)
-    groups = b * hk * ((g + gm - 1) // gm)
-    resident = int(ops.tree_decode_max_ctas(d, kv_kind, use_tc))
-    splits = _choose_splits(n, groups, resident)
     buf = _buffers(b * h, d, dev)
     need = b * hk * splits * g * (d + 4)
     if buf.scratch is None or buf.scratch.numel() < need:

@@ -481,30 +481,3 @@ def test_fp8_forward_regimes(name):
     print(f"[fp8 {name}] rel rms fp8 {err8:.3e}, bf16 {err16:.3e}, ratio {err8 / err16:.2f}")
     assert err8 <= REL_RMS_TOL, (err8, err16)
     assert err8 <= BF16_RATIO_TOL * err16, (err8, err16)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("regime", ["sink10", "peaky"])
-@pytest.mark.parametrize("tensor_core", ["auto", False])
-@pytest.mark.parametrize("b,h,hk,n,d,dtype", [(3, 8, 1, 1000, 128, torch.bfloat16), (2, 16, 2, 777, 64, torch.float16)])
-def test_tree_decode_regimes(regime, tensor_core, b, h, hk, n, d, dtype):
-    from ring_attention_pytorch_b200.ops import tree_decode_cuda as tdc
-    from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda
-
-    tdc.CONFIG["tensor_core"] = tensor_core
-    # one query per sequence: the last row of a causal prefill of n tokens
-    qs, ks, vs, _ = gdc.make_case_inputs(regime, 1, b, n, h, hk, d, dtype, "plain", True, None, seed=4)
-    q = qs[0][:, -1:].permute(0, 2, 1, 3).contiguous()      # [b, h, 1, d]
-    k, v = (t[0].permute(0, 2, 1, 3).contiguous() for t in (ks, vs))  # [b, hk, n, d]
-    out = tree_decode_cuda(q, k, v, dim_v=d)
-
-    def dense(dtype_):
-        kx = k.to(dtype_).repeat(1, h // hk, 1, 1)
-        vx = v.to(dtype_).repeat(1, h // hk, 1, 1)
-        sim = torch.einsum("bhid,bhjd->bhij", q.to(dtype_), kx) * d ** -0.5
-        return torch.einsum("bhij,bhjd->bhid", sim.softmax(-1), vx)
-
-    res = gdc.noise_bound(out, dense(torch.float32), dense(dtype))
-    _report(f"decode {regime} tc={tensor_core} d={d}", {"out": res})
-    tdc.CONFIG["tensor_core"] = "auto"
-    assert res["ok"], res

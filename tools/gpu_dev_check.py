@@ -363,6 +363,26 @@ def make_sinks(kind, qs, ks, softclamp=0.0):
     return choice[kind].contiguous()
 
 
+def decode_reference(q, k, v, sinks=None, dtype=None, batch_chunk=8):
+    """The oracle of tree decode: ``q [b, h, 1, d]`` against ``k, v [b, hk, n, d]`` (already dequantised; None or
+    n = 0 for an empty shard) with ``attention_with_positions``, computed in ``dtype`` (default fp32) and returned as
+    ``[b, h, 1, d]`` in that dtype.  It runs ``batch_chunk`` sequences at a time, so the grouped-query expansion of K
+    and V is never built for the whole batch at once (a batch-256, 8192-key cache would need 68 GB of it in fp32)."""
+    import torch
+    from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
+
+    dtype = dtype or torch.float32
+    b, h, _, d = q.shape
+    if k is None or k.shape[2] == 0:
+        return torch.zeros(b, h, 1, v.shape[-1] if v is not None else d, device=q.device, dtype=dtype)
+    sk = None if sinks is None else sinks.to(dtype)
+    outs = []
+    for i in range(0, b, batch_chunk):
+        qc, kc, vc = (t[i:i + batch_chunk].transpose(1, 2).to(dtype) for t in (q, k, v))
+        outs.append(attention_with_positions(qc, kc, vc, sinks=sk).transpose(1, 2))
+    return torch.cat(outs)
+
+
 def _case_docs(docs, b, n, world, layout, kmask, seed):
     """(per-rank document ids, per-rank key masks) of a case."""
     import torch
