@@ -14,6 +14,9 @@ tokens are appended round-robin so that the shards stay balanced.
     # no GPU
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29500 \
         examples/decode_tree_attention.py --device cpu --context 512 --batch 2 --heads 4 --kv-heads 2 --dim-head 16 --steps 8 --check
+
+    # ragged batch (seeded prompt lengths in [0, context]) and a look-back window of 4096 tokens
+    ... examples/decode_tree_attention.py --context 1048576 --batch 16 --ragged --window 4096
 """
 from __future__ import annotations
 
@@ -40,6 +43,8 @@ def parse_args(argv=None):
     ap.add_argument("--fp8", action="store_true", help="float8_e4m3fn cache with per-(batch, head) scales (CUDA only)")
     ap.add_argument("--check", action="store_true", help="compare every step with dense attention over the gathered cache")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--ragged", action="store_true", help="per-sequence prompt lengths drawn from the seed in [0, context]")
+    ap.add_argument("--window", type=int, default=None, help="look-back window: the query sees positions >= pos - W")
     return ap.parse_args(argv)
 
 
@@ -63,6 +68,8 @@ class ShardedKVCache:
 
 def run(args) -> float:
     """Inside an initialised process group.  Returns the largest error seen with ``--check`` (0.0 otherwise)."""
+    if args.ragged or args.window is not None:
+        return run_ragged(args)
     from ring_attention_pytorch_b200 import tree_attn_decode
 
     rank, world = dist.get_rank(), dist.get_world_size()
@@ -142,6 +149,114 @@ def run(args) -> float:
         kv_bytes = 2 * b * hk * cached * d * (1 if args.fp8 else (2 if cuda else 4))
         print(f"[decode] world {world}, {cached} cached tokens ({cache.len} on rank 0), batch {b}, heads {h}/{hk}: "
               f"median step {med * 1e3:.3f} ms, {b / med:.0f} tokens/s, cache read {kv_bytes / med / 1e9:.0f} GB/s whole job"
+              + (f", max |err| vs dense {worst:.2e}" if args.check else ""), flush=True)
+    return worst
+
+
+def run_ragged(args) -> float:
+    """``--ragged`` / ``--window``: every sequence has its own length, the decode passes the whole capacity buffers with
+    per-sequence ``cache_seqlens``, query positions and ``kv_pos = (rank, world)`` (token t of a sequence lives on rank
+    t % world at local slot t // world).  Slots past a sequence's length hold NaN (0x7F in e4m3): they must not matter."""
+    from ring_attention_pytorch_b200 import tree_attn_decode
+    from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
+    from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda
+
+    rank, world = dist.get_rank(), dist.get_world_size()
+    cuda = args.device == "cuda"
+    dev = torch.device("cuda", torch.cuda.current_device()) if cuda else torch.device("cpu")
+    dt = torch.bfloat16 if cuda else torch.float32
+    b, h, hk, d = args.batch, args.heads, args.kv_heads, args.dim_head
+    assert not (args.fp8 and not cuda), "the fp8 cache needs the sm_90a kernel"
+    gen = torch.Generator().manual_seed(args.seed)  # the same on every rank: lengths, queries, new tokens
+    lens = torch.full((b,), args.context, dtype=torch.int64)
+    if args.ragged:
+        lens = torch.randint(0, args.context + 1, (b,), generator=gen)
+        lens[0] = lens[0] % world  # shorter than the world: some ranks hold none of it
+    cache_dtype = torch.float8_e4m3fn if args.fp8 else dt
+
+    def local_len(n):  # tokens rank, rank + world, ... below n
+        return (n - rank + world - 1).clamp(min=0) // world
+
+    cap = (args.context + args.steps + world - 1) // world + 1
+    n0 = (args.context + world - 1) // world
+    dgen = torch.Generator(device=dev).manual_seed(args.seed * 7919 + 1 + rank)
+    pk = torch.randn(b, hk, n0, d, generator=dgen, device=dev)
+    pv = torch.randn(b, hk, n0, d, generator=dgen, device=dev)
+    k_scale = v_scale = None
+    if args.fp8:
+        k_scale = pk.abs().amax(dim=(2, 3)).reshape(-1) * (1.25 / 448.0)
+        v_scale = pv.abs().amax(dim=(2, 3)).reshape(-1) * (1.25 / 448.0)
+        dist.all_reduce(k_scale, dist.ReduceOp.MAX)
+        dist.all_reduce(v_scale, dist.ReduceOp.MAX)
+        pk, pv = pk / k_scale.view(b, hk, 1, 1), pv / v_scale.view(b, hk, 1, 1)
+    kc = torch.empty(b, hk, cap, d, dtype=cache_dtype, device=dev)
+    vc = torch.empty_like(kc)
+    for t in (kc, vc):
+        (t.view(torch.uint8).fill_(0x7F) if args.fp8 else t.fill_(float("nan")))
+    held = local_len(lens)
+    for i in range(b):
+        kc[i, :, :held[i]] = pk[i, :, :held[i]].to(cache_dtype)
+        vc[i, :, :held[i]] = pv[i, :, :held[i]].to(cache_dtype)
+    del pk, pv
+
+    def quantised(t, scale):  # what the cache stores, as fp32 (for --check)
+        t = t.to(cache_dtype).float()
+        return t * scale.view(b, hk, 1, 1) if scale is not None else t
+
+    full_k = full_v = None
+    if args.check:  # global [b, hk, max length, d] in position order, from every rank's slots
+        total = int(lens.max()) + args.steps
+        full_k, full_v = torch.zeros(b, hk, total, d), torch.zeros(b, hk, total, d)
+        parts = [None] * world
+        dist.all_gather_object(parts, (quantised(kc.float(), k_scale).cpu(), quantised(vc.float(), v_scale).cpu()))
+        for r, (pk_r, pv_r) in enumerate(parts):
+            for i in range(b):
+                m = len(range(r, int(lens[i]), world))
+                full_k[i, :, r:r + world * m:world], full_v[i, :, r:r + world * m:world] = pk_r[i, :, :m], pv_r[i, :, :m]
+
+    worst, times, seen = 0.0, [], 0
+    for _ in range(args.steps):
+        q = torch.randn(b, h, 1, d, generator=gen).to(dev, dt)
+        k_new, v_new = torch.randn(b, hk, d, generator=gen), torch.randn(b, hk, d, generator=gen)
+        if args.fp8:
+            k_new, v_new = k_new / k_scale.view(b, hk, 1).cpu(), v_new / v_scale.view(b, hk, 1).cpu()
+        mine = (lens % world == rank).nonzero().flatten()  # the new token of sequence i goes to rank lens[i] % world
+        slot = held[mine]
+        kc[mine.to(dev), :, slot.to(dev)] = k_new[mine].to(dev, cache_dtype)
+        vc[mine.to(dev), :, slot.to(dev)] = v_new[mine].to(dev, cache_dtype)
+        q_pos = lens.clone()  # the new token's position
+        lens += 1
+        held = local_len(lens)
+        kw = dict(cache_seqlens=held.to(dev, torch.int32), q_pos=q_pos.to(dev, torch.int32), window=args.window,
+                  kv_pos=(rank, world))
+        seen += int(sum(min(int(n), (args.window or int(n)) + 1) for n in lens))
+        if cuda:
+            torch.cuda.synchronize(dev)
+        t0 = time.perf_counter()
+        if args.fp8:
+            out = tree_decode_cuda(q, kc, vc, dim_v=d, k_scale=k_scale, v_scale=v_scale, **kw)
+        else:
+            out = tree_attn_decode(q, kc, vc, shard_kv_seq=False, dim_v=d, **kw)
+        if cuda:
+            torch.cuda.synchronize(dev)
+        times.append(time.perf_counter() - t0)
+        if args.check:
+            kq = quantised(k_new[:, :, None], k_scale.cpu() if k_scale is not None else None)[:, :, 0]
+            vq = quantised(v_new[:, :, None], v_scale.cpu() if v_scale is not None else None)[:, :, 0]
+            for i in range(b):
+                full_k[i, :, q_pos[i]], full_v[i, :, q_pos[i]] = kq[i], vq[i]
+                n = int(lens[i])
+                ref = attention_with_positions(q[i:i + 1].float().cpu().transpose(1, 2),
+                                               full_k[i:i + 1, :, :n].transpose(1, 2), full_v[i:i + 1, :, :n].transpose(1, 2),
+                                               q_pos=q_pos[i:i + 1], k_pos=torch.arange(n), causal=True, window=args.window)
+                worst = max(worst, float((out[i:i + 1].float().cpu() - ref.transpose(1, 2)).abs().max()))
+    if rank == 0:
+        ts = sorted(times[min(3, len(times) - 1):])
+        med = ts[len(ts) // 2]
+        kv_bytes = 2 * hk * d * (seen / args.steps) * (1 if args.fp8 else (2 if cuda else 4))
+        print(f"[decode] world {world}, ragged {args.ragged}, window {args.window}, lengths {int(lens.min())}.."
+              f"{int(lens.max())}, batch {b}, heads {h}/{hk}: median step {med * 1e3:.3f} ms, {b / med:.0f} tokens/s, "
+              f"visible cache read {kv_bytes / med / 1e9:.0f} GB/s whole job"
               + (f", max |err| vs dense {worst:.2e}" if args.check else ""), flush=True)
     return worst
 

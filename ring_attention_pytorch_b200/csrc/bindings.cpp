@@ -564,9 +564,18 @@ void acc_convert(const Tensor& acc, Tensor out, double scale) {
 // cross-rank signal, merge over NVLink loads or NVLS multimem reductions).  Every buffer is owned by the caller
 // (ops/tree_decode_cuda.py caches them), so the call allocates nothing and can be captured in a CUDA graph.
 // ---------------------------------------------------------------------------------------------
-int64_t tree_decode_max_ctas(int64_t d, int64_t kv_kind, bool tensor_core) {
-  if (tensor_core) return rab::tree_decode_tc_max_ctas((int)kv_kind, sm_count());
-  return rab::tree_decode_max_ctas((int)d, (int)kv_kind, sm_count());
+int64_t tree_decode_max_ctas(int64_t d, int64_t kv_kind, bool tensor_core, bool ranged) {
+  if (tensor_core) return rab::tree_decode_tc_max_ctas((int)kv_kind, sm_count(), ranged);
+  return rab::tree_decode_max_ctas((int)d, (int)kv_kind, sm_count(), ranged);
+}
+
+// int32 [b] on q's device (ranged decode: per-sequence cache lengths / query positions), or null
+const int* seq_vector_ptr(const c10::optional<Tensor>& t, int64_t b, const Tensor& q, const char* name) {
+  if (!t.has_value()) return nullptr;
+  TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->dim() == 1 && t->size(0) == b &&
+                  t->is_contiguous(),
+              name, " must be a contiguous int32 [batch] tensor on q's device");
+  return t->data_ptr<int>();
 }
 
 void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::optional<Tensor>& v,
@@ -574,7 +583,9 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
                  Tensor group_done, Tensor counters, at::IntArrayRef partial_ptrs, int64_t aux_local_ptr,
                  at::IntArrayRef pad_ptrs, int64_t mc_partial_ptr, int64_t mc_aux_ptr, int64_t rank, Tensor out,
                  int64_t kv_heads, int64_t splits, double scale, int64_t scale_block_keys, double eps, int64_t grid,
-                 bool tensor_core, const c10::optional<Tensor>& sinks) {
+                 bool tensor_core, const c10::optional<Tensor>& sinks, const c10::optional<Tensor>& cache_seqlens,
+                 const c10::optional<Tensor>& q_pos, int64_t window, int64_t kv_pos_offset, int64_t kv_pos_stride,
+                 double softclamp) {
   TORCH_CHECK(q.is_cuda() && q.is_contiguous() && q.dim() == 3, "q must be contiguous [b, h, d]");
   const int b = q.size(0), h = q.size(1), d = q.size(2);
   TORCH_CHECK(d == 64 || d == 128, "tree decode supports head dim 64 or 128");
@@ -650,6 +661,18 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   TORCH_CHECK(p.out_kind != 2 || out.scalar_type() == at::kFloat);
   p.eps = (float)eps;
   p.sinks = sinks_ptr(sinks, h, q);
+  p.cache_seqlens = seq_vector_ptr(cache_seqlens, b, q, "cache_seqlens");
+  p.q_pos = seq_vector_ptr(q_pos, b, q, "q_pos");
+  TORCH_CHECK(window >= 0 && window <= INT32_MAX && (window == 0 || p.q_pos != nullptr),
+              "window must be >= 0 and needs q_pos");
+  TORCH_CHECK(kv_pos_offset >= 0 && kv_pos_offset <= INT32_MAX && kv_pos_stride >= 1 && kv_pos_stride <= INT32_MAX,
+              "kv_pos needs offset >= 0 and stride >= 1");
+  TORCH_CHECK(softclamp >= 0.0, "softclamp must be >= 0");
+  p.window = (int)window;
+  p.kv_pos_offset = (int)kv_pos_offset;
+  p.kv_pos_stride = (int)kv_pos_stride;
+  p.softclamp_log2 = (float)(softclamp * 1.4426950408889634);
+  const bool ranged = p.cache_seqlens != nullptr || p.q_pos != nullptr || softclamp > 0.0;
   c10::cuda::CUDAGuard guard(q.device());
   if (tensor_core) {
     TORCH_CHECK(d == 128 && n > 0, "the tensor-core decode kernel needs head dim 128 and a non-empty shard");
@@ -666,9 +689,9 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
       return rab::make_tmap_bf16(base, 3, dims, strides, box, rab::TmapSwizzle::B128);
     };
     CUtensorMap map_k = mk(p.k), map_v = mk(p.v);
-    rab::launch_tree_decode_tc(map_k, map_v, p, (int)grid, at::cuda::getCurrentCUDAStream());
+    rab::launch_tree_decode_tc(map_k, map_v, p, (int)grid, at::cuda::getCurrentCUDAStream(), ranged);
   } else {
-    rab::launch_tree_decode(p, d, (int)grid, at::cuda::getCurrentCUDAStream());
+    rab::launch_tree_decode(p, d, (int)grid, at::cuda::getCurrentCUDAStream(), ranged);
   }
 }
 
@@ -789,8 +812,9 @@ TORCH_LIBRARY(rab, m) {
   m.def("tree_decode(Tensor q, Tensor? k, Tensor? v, Tensor? k_scale, Tensor? v_scale, Tensor(a!) scratch, Tensor(b!) "
         "group_done, Tensor(c!) counters, int[] partial_ptrs, int aux_local_ptr, int[] pad_ptrs, int mc_partial_ptr, int "
         "mc_aux_ptr, int rank, Tensor(d!) out, int kv_heads, int splits, float scale, int scale_block_keys, float eps, "
-        "int grid, bool tensor_core, Tensor? sinks=None) -> ()");
-  m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core) -> int");
+        "int grid, bool tensor_core, Tensor? sinks=None, Tensor? cache_seqlens=None, Tensor? q_pos=None, int window=0, "
+        "int kv_pos_offset=0, int kv_pos_stride=1, float softclamp=0.0) -> ()");
+  m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core, bool ranged=False) -> int");
   m.def("bwd_prep(Tensor q, Tensor o, Tensor dout, Tensor lse, Tensor(a!) qdo_buf, Tensor(b!) stat_buf, int rank, "
         "Tensor? sinks=None, Tensor(c!)? dsinks=None) -> ()");
   m.def("attn_bwd_dq(Tensor qdo_buf, Tensor kv_buf, Tensor stat_buf, Tensor? ready, int ready_target, Tensor? "

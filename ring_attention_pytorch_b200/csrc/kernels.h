@@ -192,13 +192,24 @@ struct TreeDecodeParams {
   float eps;
   const float* sinks;                 // null or fp32 [heads] attention sinks (natural log, by query head): added once,
                                       // in the cross-rank merge; the per-rank partials never contain them
+  // Ranged decode (the `ranged` kernel instantiations; ignored by the others).  Local key j of sequence b sits at
+  // global position P(j) = kv_pos_offset + kv_pos_stride * j and is visible iff
+  //   j < min(cache_seqlens[b], n)                     (cache_seqlens null: j < n)
+  //   P(j) <= q_pos[b]  and  q_pos[b] - P(j) <= window  (q_pos null: no position rule; window <= 0: no window)
+  // The visible keys form one range [lo_b, hi_b).  Unit (b, split s) covers [lo_al + s per, min(hi_b, lo_al + (s+1) per))
+  // with lo_al = lo_b rounded down to a multiple of 64, per planned over the largest span a unit can see.
+  const int* cache_seqlens;           // null or int32 [batch] keys held for each sequence (clamped to [0, n])
+  const int* q_pos;                   // null or int32 [batch] global position of each sequence's query
+  int window;
+  int kv_pos_offset, kv_pos_stride;   // >= 0, >= 1
+  float softclamp_log2;               // > 0: logits (log2 units) become c tanh(s / c) with c = softclamp * log2(e)
 };
-int tree_decode_max_ctas(int d, int kv_kind, int num_sms);
-void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream);
+int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged);
+void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream, bool ranged);
 // wgmma variant (tree_decode_tc_sm90.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 64-key box
-int tree_decode_tc_max_ctas(int kv_kind, int num_sms);
+int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged);
 void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, const TreeDecodeParams& p, int grid,
-                           cudaStream_t stream);
+                           cudaStream_t stream, bool ranged);
 
 // ------------------------------------------------------------------------------------------------
 // misc kernels (elementwise_sm90.cu)

@@ -15,6 +15,36 @@ __device__ __forceinline__ float load_q(const void* q, int kind, size_t idx) {
   return reinterpret_cast<const float*>(q)[idx];
 }
 
+// Ranged decode: the keys unit (b, split) covers, [k0, k1), and the first visible key lo (keys in [k0, lo) are masked).
+// Tiles start at lo rounded down to a multiple of TILE, so they stay aligned with the scale blocks of an fp8 cache.
+struct TdUnitRange {
+  int lo, k0, k1;
+};
+__device__ __forceinline__ long long td_floor_div(long long a, long long b) {  // b > 0, any sign of a
+  return a >= 0 ? a / b : -((-a + b - 1) / b);
+}
+template <int TILE>
+__device__ __forceinline__ TdUnitRange td_unit_range(const TreeDecodeParams& p, int b, int split) {
+  long long lo = 0, hi = p.n;
+  if (p.cache_seqlens != nullptr) hi = min(hi, (long long)p.cache_seqlens[b]);
+  long long span = p.n;  // the most keys (with tile slack) one sequence's visible range can touch
+  if (p.q_pos != nullptr) {
+    const long long rel = (long long)p.q_pos[b] - p.kv_pos_offset;  // negative: every key here lies after the query
+    hi = min(hi, td_floor_div(rel, p.kv_pos_stride) + 1);             // P(j) <= q_pos
+    if (p.window > 0) {
+      lo = max(lo, -td_floor_div((long long)p.window - rel, p.kv_pos_stride));  // q_pos - P(j) <= window
+      span = min(span, (long long)p.window / p.kv_pos_stride + TILE);
+    }
+  }
+  lo = min(lo, (long long)p.n);
+  const long long per = ((span + p.splits - 1) / p.splits + TILE - 1) / TILE * TILE;
+  TdUnitRange r;
+  r.lo = (int)lo;
+  r.k0 = (int)min((lo & ~(long long)(TILE - 1)) + split * per, (long long)p.n);
+  r.k1 = lo < hi ? (int)max(min(hi, (long long)r.k0 + per), (long long)r.k0) : r.k0;
+  return r;
+}
+
 // order-preserving map fp32 -> int32 (so that an integer max is the float max); used for the in-switch max
 __device__ __forceinline__ int float_to_ordered(float f) {
   const int i = __float_as_int(f);

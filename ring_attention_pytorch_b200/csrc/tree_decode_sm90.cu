@@ -82,7 +82,9 @@ struct KvVec<2> {
 };
 
 
-template <int D, int KV_KIND>
+// RANGED: per-sequence visible key ranges and softclamp (TreeDecodeParams).  Key loads are clamped into [lo, k1), so a
+// masked key's probability of 0 always multiplies a visible (finite) value row.
+template <int D, int KV_KIND, bool RANGED>
 __global__ void __launch_bounds__(TD_THREADS)
 tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
   using Vec = KvVec<KV_KIND>;
@@ -128,7 +130,14 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     const int g0 = zc * TD_MAX_G;
     const int g = min(TD_MAX_G, g_total - g0);
     const int per = ((p.n + p.splits - 1) / p.splits + TD_TILE - 1) / TD_TILE * TD_TILE;  // tile-aligned splits
-    const int k0 = split * per, k1 = min(p.n, k0 + per);
+    int k0 = split * per, k1 = min(p.n, k0 + per), lo = 0;
+    if constexpr (RANGED) {
+      const TdUnitRange r = td_unit_range<TD_TILE>(p, b, split);
+      k0 = r.k0;
+      k1 = r.k1;
+      lo = r.lo;
+    }
+    const float clamp_inv = RANGED && p.softclamp_log2 > 0.f ? 1.f / p.softclamp_log2 : 0.f;
 
     const float* ksb = p.k_scale ? p.k_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
     const float* vsb = p.v_scale ? p.v_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
@@ -138,6 +147,7 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     float2 qr[TD_MAX_G][EPL / 2];  // packed pairs: two lanes of a pair per dot-product step
 #pragma unroll
     for (int gi = 0; gi < TD_MAX_G; ++gi) {
+      if (RANGED && k0 >= k1) break;  // an empty unit loads nothing
 #pragma unroll
       for (int e = 0; e < EPL / 2; ++e) {
         // query head j uses kv head j % kv_heads  ->  heads {kvh, kvh + hk, ...}
@@ -157,7 +167,8 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     auto load_k = [&](int t0) {
 #pragma unroll
       for (int step = 0; step < 4; ++step) {
-        const int key = min(t0 + warp * 16 + step * 4 + sub, k1 - 1);  // clamp: loads stay in bounds
+        int key = min(t0 + warp * 16 + step * 4 + sub, k1 - 1);  // clamp: loads stay in bounds
+        if constexpr (RANGED) key = max(key, lo);
         const uint8_t* row = kbase + ((size_t)key * D + l8 * EPL) * eb;
 #pragma unroll
         for (int c = 0; c < KVEC; ++c) kraw[step][c] = *reinterpret_cast<const Raw*>(row + c * Vec::kBytes);
@@ -166,7 +177,8 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     auto load_v = [&](int t0) {
 #pragma unroll
       for (int i = 0; i < KPT; ++i) {
-        const int key = min(t0 + kgrp + i * KGROUPS, k1 - 1);
+        int key = min(t0 + kgrp + i * KGROUPS, k1 - 1);
+        if constexpr (RANGED) key = max(key, lo);
         vraw[i] = *reinterpret_cast<const Raw*>(vbase + ((size_t)key * D + chunk * 8) * eb);
       }
     };
@@ -186,7 +198,7 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
 #pragma unroll
         for (int c = 0; c < KVEC; ++c) Vec::cvt(kraw[step][c], kf + 8 * c);
         const int kl = warp * 16 + step * 4 + sub;
-        const bool live = (t0 + kl) < k1;
+        const bool live = (t0 + kl) < k1 && (!RANGED || t0 + kl >= lo);
         float part[TD_MAX_G];
 #pragma unroll
         for (int gi = 0; gi < TD_MAX_G; ++gi) {
@@ -197,7 +209,13 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
           a += __shfl_xor_sync(0xffffffffu, a, 1);
           a += __shfl_xor_sync(0xffffffffu, a, 2);
           a += __shfl_xor_sync(0xffffffffu, a, 4);
-          part[gi] = live ? a * ks : -INFINITY;
+          if constexpr (RANGED) {
+            float x = a * ks;
+            if (p.softclamp_log2 > 0.f) x = fast_tanh(x * clamp_inv) * p.softclamp_log2;
+            part[gi] = live ? x : -INFINITY;
+          } else {
+            part[gi] = live ? a * ks : -INFINITY;
+          }
         }
         if (l8 == 0) *reinterpret_cast<float4*>(&s_s[par][kl][0]) = make_float4(part[0], part[1], part[2], part[3]);
       }
@@ -356,32 +374,29 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
   td_cross_rank_merge<D>(p, cs, total_units);
 }
 
+template <bool RANGED>
+const void* pick_td(int d, int kv_kind) {
+  if (d == 128) {
+    if (kv_kind == 0) return (const void*)tree_decode_kernel<128, 0, RANGED>;
+    if (kv_kind == 1) return (const void*)tree_decode_kernel<128, 1, RANGED>;
+    return (const void*)tree_decode_kernel<128, 2, RANGED>;
+  }
+  if (kv_kind == 0) return (const void*)tree_decode_kernel<64, 0, RANGED>;
+  if (kv_kind == 1) return (const void*)tree_decode_kernel<64, 1, RANGED>;
+  return (const void*)tree_decode_kernel<64, 2, RANGED>;
+}
 
 }  // namespace
 
-int tree_decode_max_ctas(int d, int kv_kind, int num_sms) {
+int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged) {
   int per_sm = 0;
-  const void* fn = nullptr;
-#define RAB_TD_PICK(DD, KK) fn = (const void*)tree_decode_kernel<DD, KK>
-  if (d == 128) {
-    if (kv_kind == 0) RAB_TD_PICK(128, 0); else if (kv_kind == 1) RAB_TD_PICK(128, 1); else RAB_TD_PICK(128, 2);
-  } else {
-    if (kv_kind == 0) RAB_TD_PICK(64, 0); else if (kv_kind == 1) RAB_TD_PICK(64, 1); else RAB_TD_PICK(64, 2);
-  }
-#undef RAB_TD_PICK
+  const void* fn = ranged ? pick_td<true>(d, kv_kind) : pick_td<false>(d, kv_kind);
   cuda_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, TD_THREADS, 0), "tree_decode occupancy");
   return per_sm * num_sms;
 }
 
-void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream) {
-  const void* fn = nullptr;
-#define RAB_TD_PICK(DD, KK) fn = (const void*)tree_decode_kernel<DD, KK>
-  if (d == 128) {
-    if (p.kv_kind == 0) RAB_TD_PICK(128, 0); else if (p.kv_kind == 1) RAB_TD_PICK(128, 1); else RAB_TD_PICK(128, 2);
-  } else {
-    if (p.kv_kind == 0) RAB_TD_PICK(64, 0); else if (p.kv_kind == 1) RAB_TD_PICK(64, 1); else RAB_TD_PICK(64, 2);
-  }
-#undef RAB_TD_PICK
+void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream, bool ranged) {
+  const void* fn = ranged ? pick_td<true>(d, p.kv_kind) : pick_td<false>(d, p.kv_kind);
   void* args[] = {(void*)&p};
   // cooperative: the grid barrier and the cross-rank waits need every CTA of the grid to be resident
   cuda_check(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(TD_THREADS), args, 0, stream), "tree_decode launch");

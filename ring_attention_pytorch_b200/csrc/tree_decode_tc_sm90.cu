@@ -81,8 +81,10 @@ __device__ __forceinline__ void widen_fp8_tile(const uint8_t* src, uint8_t* dst,
   }
 }
 
-// KVK: 0 bf16, 1 fp16, 2 fp8-e4m3 cache.  NH: query heads per unit (MMA N).
-template <int KVK, int NH>
+// KVK: 0 bf16, 1 fp16, 2 fp8-e4m3 cache.  NH: query heads per unit (MMA N).  RANGED: per-sequence visible key ranges
+// and softclamp (TreeDecodeParams); V rows of invisible keys in a unit's boundary tiles are zeroed in shared memory,
+// since a probability of 0 does not cancel a NaN value row inside the MMA.
+template <int KVK, int NH, bool RANGED>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                       const __grid_constant__ TreeDecodeParams p) {
@@ -132,7 +134,13 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
     const int g0 = zc * NH;
     const int g = min(NH, g_total - g0);
     const int per = ((p.n + p.splits - 1) / p.splits + TC_TILE - 1) / TC_TILE * TC_TILE;  // tile-aligned splits
-    const int k0 = split * per, k1 = min(p.n, k0 + per);
+    int k0 = split * per, k1 = min(p.n, k0 + per), lo = 0;
+    if constexpr (RANGED) {
+      const TdUnitRange r = td_unit_range<TC_TILE>(p, b, split);
+      k0 = r.k0;
+      k1 = r.k1;
+      lo = r.lo;
+    }
     const int ntiles = k0 < k1 ? (k1 - k0 + TC_TILE - 1) / TC_TILE : 0;
     const float* ksb = p.k_scale ? p.k_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
     const float* vsb = p.v_scale ? p.v_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
@@ -156,7 +164,7 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
       for (int i = 0; i < min(TC_NST, ntiles); ++i) issue(i);
 
     // Q^T as the B operand (16 bit, zero for padded heads); the softmax scale is applied to the logits
-    for (int i = tid; i < NH * D / 2; i += TC_THREADS) {
+    for (int i = tid; i < ((!RANGED || ntiles > 0) ? NH * D / 2 : 0); i += TC_THREADS) {
       const int gi = i / (D / 2), c = 2 * (i % (D / 2));
       float a = 0.f, bq = 0.f;
       if (gi < g) {
@@ -180,6 +188,7 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
       mr[c] = -INFINITY;
       lp[c] = 0.f;
     }
+    const float clamp_inv = RANGED && p.softclamp_log2 > 0.f ? 1.f / p.softclamp_log2 : 0.f;
     const uint64_t q_desc = gmma_desc(kmaj, sm.q[0]);
     const uint64_t p_desc = gmma_desc(kmaj, sm.p);
 
@@ -196,6 +205,17 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
         named_bar_sync(1, TC_THREADS);
         kt = sm.kc;
         vt = sm.vc;
+      }
+      if constexpr (RANGED) {
+        if (t0 < lo || t0 + TC_TILE > k1) {  // boundary tile: zero the V rows of the keys outside [lo, k1)
+          uint8_t* vz = KV8 ? sm.vc : sm.v[st];
+          for (int i = tid; i < TC_TILE * 16; i += TC_THREADS) {
+            const int row = i / 16, c = i % 16, key = t0 + row;
+            if (key < lo || key >= k1)
+              *reinterpret_cast<uint4*>(vz + (c / 8) * TC_SUB + row * 128 + (c % 8) * 16) = make_uint4(0u, 0u, 0u, 0u);
+          }
+          fence_proxy_async_shared();  // ordered before the P V wgmma by the barrier after P is written
+        }
       }
       // ---- S^T = K Q^T --------------------------------------------------------------------------------------------
       float s[NH / 2];
@@ -218,7 +238,13 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
 #pragma unroll
       for (int i = 0; i < NH / 2; ++i) {
         const int key = t0 + r_lo + 8 * ((i >> 1) & 1);
-        s[i] = key < k1 ? s[i] * ks : -INFINITY;
+        if constexpr (RANGED) {
+          float x = s[i] * ks;
+          if (p.softclamp_log2 > 0.f) x = fast_tanh(x * clamp_inv) * p.softclamp_log2;
+          s[i] = (key >= lo && key < k1) ? x : -INFINITY;  // a select: a NaN logit of a masked key goes too
+        } else {
+          s[i] = key < k1 ? s[i] * ks : -INFINITY;
+        }
         const int c = 2 * (i / 4) + (i & 1);
         cmax[c] = fmaxf(cmax[c], s[i]);
       }
@@ -370,13 +396,18 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
   td_cross_rank_merge<D>(p, cs, total_units);
 }
 
-template <int KVK>
+template <int KVK, bool RANGED>
 const void* tc_ptr_nh(bool small_group) {
-  return small_group ? (const void*)tree_decode_tc_kernel<KVK, 8> : (const void*)tree_decode_tc_kernel<KVK, 16>;
+  return small_group ? (const void*)tree_decode_tc_kernel<KVK, 8, RANGED>
+                     : (const void*)tree_decode_tc_kernel<KVK, 16, RANGED>;
 }
-const void* pick_tc(int kv_kind, bool small_group) {
-  if (kv_kind == 2) return tc_ptr_nh<2>(small_group);
-  return kv_kind == 1 ? tc_ptr_nh<1>(small_group) : tc_ptr_nh<0>(small_group);
+template <bool RANGED>
+const void* pick_tc_r(int kv_kind, bool small_group) {
+  if (kv_kind == 2) return tc_ptr_nh<2, RANGED>(small_group);
+  return kv_kind == 1 ? tc_ptr_nh<1, RANGED>(small_group) : tc_ptr_nh<0, RANGED>(small_group);
+}
+const void* pick_tc(int kv_kind, bool small_group, bool ranged) {
+  return ranged ? pick_tc_r<true>(kv_kind, small_group) : pick_tc_r<false>(kv_kind, small_group);
 }
 size_t tc_smem(int kv_kind, bool small_group) {
   size_t s;
@@ -387,9 +418,9 @@ size_t tc_smem(int kv_kind, bool small_group) {
 
 }  // namespace
 
-int tree_decode_tc_max_ctas(int kv_kind, int num_sms) {
+int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged) {
   const bool small = false;  // the 16-head variant: the larger shared-memory footprint bounds residency
-  const void* fn = pick_tc(kv_kind, small);
+  const void* fn = pick_tc(kv_kind, small, ranged);
   const size_t smem = tc_smem(kv_kind, small);
   cuda_check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tree_decode_tc smem attr");
   int per_sm = 0;
@@ -398,9 +429,9 @@ int tree_decode_tc_max_ctas(int kv_kind, int num_sms) {
 }
 
 void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, const TreeDecodeParams& p, int grid,
-                           cudaStream_t stream) {
+                           cudaStream_t stream, bool ranged) {
   const bool small = p.heads / p.kv_heads <= 8;
-  const void* fn = pick_tc(p.kv_kind, small);
+  const void* fn = pick_tc(p.kv_kind, small, ranged);
   const size_t smem = tc_smem(p.kv_kind, small);
   cuda_check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tree_decode_tc smem attr");
   void* args[] = {(void*)&map_k, (void*)&map_v, (void*)&p};

@@ -22,17 +22,43 @@ import torch.distributed as dist
 from torch import Tensor
 
 from ring_attention_pytorch_b200.parallel.distributed import default, exists, get_rank, get_world_size, is_distributed
-from ring_attention_pytorch_b200.utils.validate import check_sinks, typecheck
+from ring_attention_pytorch_b200.utils.validate import check_decode_ranges, check_sinks, typecheck
 
 
-def _local_attention(q: Tensor, k: Tensor, v: Tensor):
-    """q [b,h,1,d], k [b,hk,n,d], v [b,hk,n,dv] -> (out [b,h,1,dv] fp32, lse [b,h,1,1] fp32)."""
+def _visible_keys(n: int, cache_seqlens: Optional[Tensor], q_pos: Optional[Tensor], window: Optional[int],
+                  kv_pos: tuple[int, int], b: int, device) -> Tensor:
+    """bool [b, n]: local key j of sequence b is visible (see :func:`tree_attn_decode`)."""
+    j = torch.arange(n, device=device, dtype=torch.int64)
+    vis = torch.ones(b, n, dtype=torch.bool, device=device)
+    if cache_seqlens is not None:
+        vis &= j[None] < cache_seqlens.to(torch.int64)[:, None]
+    if q_pos is not None:
+        rel = q_pos.to(torch.int64)[:, None] - (kv_pos[0] + kv_pos[1] * j)[None]
+        vis &= rel >= 0
+        if window is not None and window > 0:
+            vis &= rel <= window
+    return vis
+
+
+def _local_attention(q: Tensor, k: Tensor, v: Tensor, visible: Optional[Tensor] = None, softclamp_value: float = 0.0):
+    """q [b,h,1,d], k [b,hk,n,d], v [b,hk,n,dv] -> (out [b,h,1,dv] fp32, lse [b,h,1,1] fp32).  ``visible`` (bool
+    [b, n]) masks keys; a row that sees none gives out 0 and the finite sentinel lse ``-finfo.max``, so that the
+    cross-rank merge of a row empty on every rank computes exp(0), never -inf - -inf."""
     b, h, _, d = q.shape
     hk = k.shape[1]
     g = h // hk
     scale = d ** -0.5
     qf = q.float().view(b, g, hk, 1, d)  # query head j uses kv head j % hk
     sim = torch.einsum("bghid,bhjd->bghij", qf, k.float()) * scale
+    if visible is not None:
+        if softclamp_value > 0:
+            sim = (sim / softclamp_value).tanh() * softclamp_value
+        sim = sim.masked_fill(~visible[:, None, None, None, :], -float("inf"))
+        lse = sim.logsumexp(dim=-1, keepdim=True)
+        lse = torch.where(lse == -float("inf"), torch.full_like(lse, -torch.finfo(torch.float32).max), lse)
+        vf = v.float().masked_fill(~visible[:, None, :, None], 0.0)  # 0 * NaN is NaN: invisible rows may hold anything
+        out = torch.einsum("bghij,bhjd->bghid", (sim - lse).exp(), vf)
+        return out.reshape(b, h, 1, -1), lse.reshape(b, h, 1, 1)
     lse = sim.logsumexp(dim=-1, keepdim=True)
     attn = (sim - lse).exp()
     out = torch.einsum("bghij,bhjd->bghid", attn, v.float())
@@ -50,6 +76,11 @@ def tree_attn_decode(
     use_triton: Optional[bool] = None,
     dim_v: Optional[int] = None,
     sinks: Optional[Tensor] = None,
+    cache_seqlens: Optional[Tensor] = None,
+    q_pos: Optional[Tensor] = None,
+    window: Optional[int] = None,
+    softclamp_value: float = 0.0,
+    kv_pos: Optional[tuple[int, int]] = None,
 ) -> Tensor:
     """Returns ``[b, h, 1, dv]`` in ``q.dtype``.
 
@@ -60,19 +91,41 @@ def tree_attn_decode(
 
     ``sinks`` (floating ``[h]``): learned attention sinks, one logit per query head with a zero value vector.  The
     softmax runs over the keys of every rank and the sink, which is added once, in the cross-rank merge.
+
+    Ragged and windowed decode: key ``j`` of a rank's K/V sits at global position ``P(j) = offset + stride * j`` and is
+    visible to sequence ``b`` iff ``j < cache_seqlens[b]`` (int32 ``[b]``, the keys held), ``P(j) <= q_pos[b]``
+    (integer ``[b]``) and, with ``window > 0``, ``q_pos[b] - P(j) <= window`` -- the look-back rule of the ring op.
+    With ``shard_kv_seq=True`` the lengths and positions are global and each rank derives its own from its
+    ``chunk`` (``offset = rank * chunk``, ``stride = 1``); with ``shard_kv_seq=False`` they are this rank's and
+    ``kv_pos = (offset, stride)`` places its keys (required with ``q_pos`` on more than one rank; e.g. ``(rank,
+    world)`` for round-robin appends).  ``softclamp_value > 0``: logits ``c * tanh(s / c)`` (the sink is not clamped).
+    A row that sees no key on any rank and has no sink gives 0.
     """
     assert not (exists(k) ^ exists(v)), "keys and values are either both None, or both present"
     dtype = q.dtype
     b, h = q.shape[:2]
     check_sinks(sinks, h, q.device, name="tree_attn_decode")
+    check_decode_ranges(b, q.device, cache_seqlens, q_pos, window, kv_pos, softclamp_value, name="tree_attn_decode")
+    ranged = exists(cache_seqlens) or exists(q_pos) or softclamp_value > 0
     if exists(v):
         dim_v = v.shape[-1]
 
     if shard_kv_seq:
         assert exists(k), "keys and values must be passed if not already sharded across sequence"
+        if exists(kv_pos):
+            raise ValueError("tree_attn_decode: kv_pos is derived from the chunk with shard_kv_seq=True")
         rank, world = get_rank(), get_world_size()
         ks, vs = k.chunk(world, dim=-2), v.chunk(world, dim=-2)
         k, v = (ks[rank], vs[rank]) if rank < len(ks) else (None, None)
+        if ranged and exists(k):
+            offset = rank * ks[0].shape[-2]
+            kv_pos = (offset, 1)
+            if exists(cache_seqlens):
+                cache_seqlens = (cache_seqlens - offset).clamp(0, k.shape[-2]).to(torch.int32)
+    elif exists(q_pos) and not exists(kv_pos) and is_distributed() and get_world_size() > 1:
+        raise ValueError("tree_attn_decode: kv_pos = (offset, stride) of this rank's keys is required with q_pos "
+                         "when the cache is sharded over more than one rank")
+    kv_pos = default(kv_pos, (0, 1))
     assert exists(dim_v), "dim_v is required when this rank holds no keys"
 
     use_kernel = default(use_triton, q.is_cuda)
@@ -81,9 +134,15 @@ def tree_attn_decode(
     if use_kernel:
         from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda
 
+        if ranged:
+            return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps, sinks=sinks, cache_seqlens=cache_seqlens, q_pos=q_pos,
+                                    window=window, kv_pos=kv_pos, softclamp_value=softclamp_value).to(dtype)
         return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps, sinks=sinks).to(dtype)
 
-    if exists(k) and k.shape[-2] > 0:
+    if exists(k) and k.shape[-2] > 0 and ranged:
+        visible = _visible_keys(k.shape[-2], cache_seqlens, q_pos, window, kv_pos, b, q.device)
+        local_out, lse = _local_attention(q, k, v, visible, softclamp_value)
+    elif exists(k) and k.shape[-2] > 0:
         local_out, lse = _local_attention(q, k, v)
     else:
         local_out = q.new_zeros((b, h, 1, dim_v), dtype=torch.float32)

@@ -19,6 +19,7 @@ from torch import Tensor
 
 from ring_attention_pytorch_b200.ops import _ext
 from ring_attention_pytorch_b200.parallel.distributed import get_rank, get_world_size, is_distributed
+from ring_attention_pytorch_b200.utils.validate import check_decode_ranges
 
 LAUNCHES = {"count": 0}
 # nvls "auto": use the NVSwitch multicast mapping when torch's symmetric memory can provide one, else NVLink peer loads
@@ -27,6 +28,7 @@ LAUNCHES = {"count": 0}
 CONFIG = {"nvls": "auto", "tensor_core": "auto"}
 K_MAX_WORLD = 16
 PAD_WORDS = 2 * K_MAX_WORLD  # two signal rounds
+TILE = 64  # keys per tile in both kernels; unit ranges start on a multiple of it
 
 
 def _choose_splits(n: int, groups: int, resident_ctas: int) -> int:
@@ -45,14 +47,31 @@ class DecodePlan:
     splits: int        # key splits per group
 
 
-def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int) -> DecodePlan:
-    """The kernel and the work split a decode call of these sizes gets (``kv_kind``: 0 bf16, 1 fp16, 2 fp8 cache)."""
+def decode_span(n: int, window: Optional[int] = None, kv_pos_stride: int = 1) -> int:
+    """The most keys, with the up-to-63-key slack of tile alignment, that one sequence's visible range can touch: the
+    ranged kernels split this span, not ``n``.  With a look-back window a query sees at most ``window // stride + 1``
+    local keys, so the splits cover O(window) keys."""
+    if window is None or window <= 0:
+        return n
+    return min(n, window // kv_pos_stride + TILE)
+
+
+def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int, *, ranged: bool = False,
+                span: Optional[int] = None) -> DecodePlan:
+    """The kernel and the work split a decode call of these sizes gets (``kv_kind``: 0 bf16, 1 fp16, 2 fp8 cache).
+    ``ranged``: the instantiations with per-sequence key ranges / softclamp; ``span`` (default ``n``): the keys the
+    splits are planned over (:func:`decode_span`)."""
     tc = CONFIG["tensor_core"]
     use_tc = tc in ("auto", True, "on") and d == 128 and n >= 1
     g = h // hk
     gm = (8 if g <= 8 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: MMA N)
     groups = b * hk * ((g + gm - 1) // gm)
     resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc))
+    if ranged:
+        # the splits follow the plain kernel's residency, so full-length ranges split exactly like the plain call;
+        # the grid is bounded by the ranged kernel's own residency (cooperative launch)
+        splits = _choose_splits(n if span is None else span, groups, resident)
+        return DecodePlan(use_tc, groups, int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc, True)), splits)
     return DecodePlan(use_tc, groups, resident, _choose_splits(n, groups, resident))
 
 
@@ -167,6 +186,11 @@ def tree_decode_cuda(
     scale_block_keys: int = 0,
     out: Optional[Tensor] = None,
     sinks: Optional[Tensor] = None,
+    cache_seqlens: Optional[Tensor] = None,
+    q_pos: Optional[Tensor] = None,
+    window: Optional[int] = None,
+    kv_pos: Tuple[int, int] = (0, 1),
+    softclamp_value: float = 0.0,
 ) -> Tensor:
     """q [b, h, 1, d] (bf16 / fp16 / fp32); k, v [b, hk, n, d] this rank's shard (bf16 / fp16 / float8_e4m3fn) or None.
     k / v may be the filled prefix ``cache[:, :, :n]`` of a larger ``[b, hk, capacity, d]`` buffer: the tensor-core kernel
@@ -177,9 +201,18 @@ def tree_decode_cuda(
     (a multiple of 64).  ``out`` ([b, h, 1, d]) may be passed to make the call allocation free (CUDA graphs).
     ``sinks`` (``[h]``, fp32 contiguous for an allocation-free call): learned attention sinks, added once, in the
     kernel's cross-rank merge.  Returns [b, h, 1, d] in q's dtype.
+
+    Ragged and windowed decode.  Local key ``j`` sits at global position ``P(j) = kv_pos[0] + kv_pos[1] * j`` and is
+    visible iff ``j < min(cache_seqlens[b], n)`` (int32 ``[b]``; None: every key), ``P(j) <= q_pos[b]`` (integer
+    ``[b]``; int32 keeps the call allocation free) and, with ``window > 0``, ``q_pos[b] - P(j) <= window``.  The
+    kernel derives each sequence's key range from the device tensors, so a decode loop can update them in place and
+    replay a captured graph; the whole ``[b, hk, capacity, d]`` buffers may be passed.  ``softclamp_value > 0`` turns
+    the logits into ``c * tanh(s / c)`` (not the sink).  A row that sees no key and has no sink gives 0.
     """
     ops = _ext.ops()
     b, h, _, d = q.shape
+    check_decode_ranges(b, q.device, cache_seqlens, q_pos, window, kv_pos, softclamp_value, name="tree_decode_cuda")
+    ranged = cache_seqlens is not None or q_pos is not None or softclamp_value > 0
     assert dim_v == d, "the decode kernel assumes dim_v == dim_qk"
     dev = q.device
     q3 = q.reshape(b, h, d)
@@ -196,7 +229,10 @@ def tree_decode_cuda(
         k = v = None
     g = h // hk
     kv_kind = 0 if k is None or k.dtype == torch.bfloat16 else (1 if k.dtype == torch.float16 else 2)
-    plan = decode_plan(b, h, hk, n, d, kv_kind)
+    if ranged:
+        plan = decode_plan(b, h, hk, n, d, kv_kind, ranged=True, span=decode_span(n, window, int(kv_pos[1])))
+    else:
+        plan = decode_plan(b, h, hk, n, d, kv_kind)
     use_tc, groups, resident, splits = plan.tensor_core, plan.groups, plan.resident, plan.splits
     if k is not None and not (use_tc and _is_cache_prefix(k) and v.stride() == k.stride()):
         k, v = k.contiguous(), v.contiguous()  # no-op for dense inputs
@@ -213,8 +249,18 @@ def tree_decode_cuda(
         sinks = sinks.float().contiguous()
     units = groups * splits if n > 0 else 0
     grid = max(1, min(resident, max(units, (b * h + 3) // 4)))
-    ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
-                    buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out.view(b, h, d), hk,
-                    splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks)
+    if ranged:
+        if q_pos is not None and q_pos.dtype != torch.int32:
+            q_pos = q_pos.to(torch.int32)
+        ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
+                        buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out.view(b, h, d),
+                        hk, splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks,
+                        cache_seqlens.contiguous() if cache_seqlens is not None else None, q_pos.contiguous()
+                        if q_pos is not None else None, window or 0, int(kv_pos[0]), int(kv_pos[1]),
+                        float(softclamp_value))
+    else:
+        ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
+                        buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out.view(b, h, d),
+                        hk, splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks)
     LAUNCHES["count"] += 1
     return out

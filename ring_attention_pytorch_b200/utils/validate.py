@@ -71,6 +71,34 @@ def check_sinks(sinks: Optional[Tensor], heads: int, device, *, name: str = "att
         raise ValueError(f"{name}: sinks must live on {device}, got {sinks.device}")
 
 
+def check_decode_ranges(batch: int, device, cache_seqlens: Optional[Tensor], q_pos: Optional[Tensor],
+                        window: Optional[int], kv_pos, softclamp_value: float, *, name: str = "decode") -> None:
+    """Per-sequence key ranges of a decode call: ``cache_seqlens`` int32 ``[batch]``, ``q_pos`` integer ``[batch]``,
+    both on the inputs' device; ``window`` (>= 0) only with ``q_pos``; ``kv_pos = (offset >= 0, stride >= 1)``;
+    ``softclamp_value >= 0``.  Values inside the tensors are not read (no host sync): lengths are clamped to the cache."""
+    for nm, t, dtypes in (("cache_seqlens", cache_seqlens, (torch.int32,)),
+                          ("q_pos", q_pos, (torch.int8, torch.int16, torch.int32, torch.int64, torch.uint8))):
+        if t is None:
+            continue
+        if not torch.is_tensor(t) or t.dim() != 1 or t.shape[0] != batch:
+            raise ValueError(f"{name}: {nm} must be a 1-D tensor of one entry per sequence [{batch}], got "
+                             f"{tuple(t.shape) if torch.is_tensor(t) else type(t)}")
+        if t.dtype not in dtypes:
+            raise ValueError(f"{name}: {nm} must be {'int32' if len(dtypes) == 1 else 'an integer tensor'}, got {t.dtype}")
+        if t.device != torch.device(device):
+            raise ValueError(f"{name}: {nm} must live on {device}, got {t.device}")
+    if window is not None:
+        if q_pos is None:
+            raise ValueError(f"{name}: a look-back window needs q_pos, the position of each sequence's query")
+        if window < 0 or window >= 2 ** 31:
+            raise ValueError(f"{name}: window must be in [0, 2**31), got {window}")
+    if kv_pos is not None:
+        if len(kv_pos) != 2 or not 0 <= int(kv_pos[0]) < 2 ** 31 or not 1 <= int(kv_pos[1]) < 2 ** 31:
+            raise ValueError(f"{name}: kv_pos must be (offset >= 0, stride >= 1), got {tuple(kv_pos)}")
+    if not softclamp_value >= 0.0:
+        raise ValueError(f"{name}: softclamp_value must be >= 0, got {softclamp_value}")
+
+
 def check_fp8_attention_inputs(q: Tensor, k: Tensor, v: Tensor, q_descale, k_descale, v_descale,
                                mask: Optional[Tensor] = None, *, name: str = "attention",
                                rotary_freqs: Optional[Tensor] = None, sinks: Optional[Tensor] = None) -> None:
