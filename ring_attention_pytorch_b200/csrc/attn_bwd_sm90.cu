@@ -6,17 +6,22 @@
 //   attn_bwd_dkv_kernel  (KV-stationary) per 128-key tile (64 keys per consumer warpgroup), for every query tile
 //        (64 rows) that can see it:  S^T = K Q^T, dP^T = V dO^T  ->  P^T, dS^T in registers
 //        dV += P^T dO, dK += dS^T Q (Q / dO read MN-major).
-//        ONE_PASS (the ring backward of attn_bwd_ring): the warpgroup also writes dS^T to shared memory and computes
-//        dQ = dS K for its 64 keys (dS read MN-major), added into the fp32 dQ accumulator with vector reductions.
+//        ONE_PASS (the ring backward of attn_bwd_ring): both warpgroups write their dS^T half into one shared
+//        [128 keys][64 queries] tile; dK += dS^T Q reads it from there, and warpgroup w computes
+//        dQ[64 q][64 w .. 64 w + 63] = dS K over all 128 keys, staged in shared memory and added into the fp32 dQ
+//        accumulator with TMA tensor reductions.
 //        dK / dV then go out either as 16 bit (single rank) or added into the K/V owner's fp32 accumulators (ring).
 //
 // Roles (384 threads, 1 CTA / SM, persistent): warps 0-3 / 4-7 consumer warpgroups (issue their own wgmma), warp 8
-// TMA producer, warps 9-11 idle.  The softmax scale is folded into the dQ / dK epilogues.
+// TMA producer (it also walks the tile schedule and hands each streamed tile to the consumers), warps 9-11 idle.
+// The softmax scale is folded into the dQ / dK epilogues.
 //
 // Inputs of the two-kernel pass are the *gathered* ring buffers (see kernels.h); remote slots are published through
 // ready flags.
 #include <cuda_fp16.h>
 
+// no printf in the watchdogs: a function call would serialize the wgmma of these kernels (see ptx.cuh)
+#define RAB_WATCHDOG_PRINTF 0
 #include "attn_common.cuh"
 
 namespace rab {
@@ -346,6 +351,14 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qd, const __grid_cons
 // =================================================================================================
 constexpr int QST = 3;
 
+// What the producer hands the consumers with each Q / dO stage (written before its arrive on qd_full).
+struct DkvTileRec {
+  int idx;    // query tile index; -1 marks the end of the item (the stage then carries no data)
+  int rep;    // query head inside the GQA group
+  int owner;  // ring rank of the queries
+  int part;   // the tile pair needs per-element masking
+};
+
 template <int D>
 struct DkvSmem {
   static constexpr int NSUB = D / 64;
@@ -355,12 +368,18 @@ struct DkvSmem {
   alignas(1024) uint8_t v[KV_TILE];
   alignas(1024) uint8_t q[QST][Q_TILE];
   alignas(1024) uint8_t dout[QST][Q_TILE];
-  alignas(1024) uint8_t ds[2][SUB64];  // dS^T [64 keys][64 queries] of warpgroup w (one-pass mode)
+  // one-pass mode: dS^T [128 keys][64 queries] (warpgroup w writes keys 64 w ..), double buffered so that a
+  // warpgroup can write the next tile's half while the other one's dQ wgmma still reads this one
+  alignas(1024) uint8_t ds[2][SUB128];
+  // one-pass mode: dQ [64 q][64 d] of warpgroup w as two [64 q][32 d] boxes (128B swizzle), source of the tensor reduce
+  alignas(1024) float dq_stage[2][64 * 64];
   alignas(16) float lse2[QST][64];
   alignas(16) float delta[QST][64];
+  DkvTileRec rec[QST];
   uint64_t kv_full, kv_empty;
   uint64_t qd_full[QST], qd_empty[QST];
 };
+static_assert(sizeof(DkvSmem<128>) + 1024 <= 227 * 1024, "DkvSmem exceeds the opt-in shared memory of an SM");
 
 struct DkvItem {
   int owner, b, kvh, key0;  // owner: ring rank whose keys the item holds
@@ -457,13 +476,22 @@ __device__ __forceinline__ void dkv_producer(DkvSmem<D>& sm, const P& p, const C
     DkvScan<DOCS> scan;
     dkv_init_scan<ONE_PASS, DOCS>(scan, p, it);
     ScanTile t;
-    while (scan.next(lane, t)) {
-      if (lane == 0) {
+    bool more = true;
+    while (more) {
+      more = scan.next(lane, t);
+      if (lane == 0 && !more) {  // end of the item: an empty stage whose record tells the consumers to move on
+        const uint32_t st = n_tile % QST, ph = (n_tile / QST) & 1;
+        mbar_wait(&sm.qd_empty[st], ph ^ 1, 810 + st);
+        sm.rec[st] = DkvTileRec{-1, 0, 0, 0};
+        mbar_arrive(&sm.qd_full[st]);
+      }
+      if (lane == 0 && more) {
         if (!ONE_PASS) wait_owner_ready(p, t.owner, ready_mask, 802);
         const uint32_t st = n_tile % QST, ph = (n_tile / QST) & 1;
         const int bh = it.b * p.heads + t.rep * p.kv_heads + it.kvh;
         const int slot = ONE_PASS ? 0 : t.owner * 2;  // the one-pass kernel reads the local [2][b*h][n_q][d] Q / dO
         mbar_wait(&sm.qd_empty[st], ph ^ 1, 810 + st);
+        sm.rec[st] = DkvTileRec{t.idx, t.rep, t.owner, t.part[0] ? 1 : 0};
         mbar_expect_tx(&sm.qd_full[st], 2 * Q_TILE + 2 * 64 * 4);
 #pragma unroll
         for (int s = 0; s < NSUB; ++s) {
@@ -483,15 +511,17 @@ __device__ __forceinline__ void dkv_producer(DkvSmem<D>& sm, const P& p, const C
 
 // Thread layout: rows (keys) r_lo and r_lo + 8 of the warpgroup's 64 keys, query columns 8 j + cq (+1).
 template <int D, bool BF16, bool ONE_PASS, bool DOCS, class P>
-__device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const int W) {
+__device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const CUtensorMap* map_dq, const int W) {
   constexpr uint64_t qmn = gmma_desc_static(SUB64, 1024);   // Q / dO as MN-major B (K = queries, N = d)
   constexpr uint64_t kmn = gmma_desc_static(SUB128, 1024);  // K as MN-major B of dQ = dS K (K = keys, N = d)
   constexpr uint64_t dsmn = gmma_desc_static(SUB64, 1024);  // dS^T [key][q] as MN-major A of dQ = dS K
   const int wg_tid = threadIdx.x - 128 * W;
+  const int wg_warp = wg_tid / 32;
   const int lane = lane_id();
-  const int r_lo = (wg_tid / 32) * 16 + lane / 4;
+  const int r_lo = wg_warp * 16 + lane / 4;
   const int cq = 2 * (lane % 4);
   uint32_t n_item = 0, n_tile = 0;
+  uint32_t n_ds = 0;  // tiles computed so far: selects the dS^T buffer (one-pass mode)
 
   const bool clamp = p.softclamp > 0.f;
   const float mul = clamp ? 1.f : p.scale * kLog2e;
@@ -529,15 +559,18 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
 
-    DkvScan<DOCS> scan;
-    dkv_init_scan<ONE_PASS, DOCS>(scan, p, it);
-    ScanTile t;
     bool any = false;
-    while (scan.next(lane, t)) {
+    while (true) {
       const uint32_t st = n_tile % QST, ph = (n_tile / QST) & 1;
       n_tile++;
-      any = true;
       mbar_wait(&sm.qd_full[st], ph, 910 + W);
+      const DkvTileRec t = sm.rec[st];
+      if (t.idx < 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sm.qd_empty[st]);
+        break;
+      }
+      any = true;
       float s[32], dp[32];
       const uint64_t q_desc = gmma_desc(KMAJ, sm.q[st]);
       const uint64_t do_desc = gmma_desc(KMAJ, sm.dout[st]);
@@ -563,7 +596,7 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
       const int a0 = p.pos.base0[t.owner] + p.pos.stride * c0 + p.q_pos_offset;
       const int a1 = p.pos.base1[t.owner] + p.pos.stride * (c0 - p.pos.seg_len) + p.q_pos_offset;
       const int ncols = p.n_q - c0;
-      const bool part = t.part[0];
+      const bool part = t.part != 0;
       uint32_t pa[16], da[16];
 #pragma unroll
       for (int i = 0; i < 32; i += 2) {
@@ -601,18 +634,6 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
         pa[i / 2] = pack16<BF16>(pp[0], pp[1]);
         da[i / 2] = pack16<BF16>(dd[0], dd[1]);
       }
-      if constexpr (ONE_PASS) {
-        // dS^T -> shared memory ([key][query], 128B swizzle) as the MN-major A operand of dQ = dS K
-        uint8_t* ds = sm.ds[W];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int row = r_lo + 8 * (i & 1);
-          const int col = 8 * (i / 2) + cq;
-          *reinterpret_cast<uint32_t*>(ds + sw128_off(row, col)) = da[i];
-        }
-        fence_proxy_async_shared();
-        named_bar_sync(1 + W, 128);
-      }
       const uint64_t qb_desc = gmma_desc(qmn, sm.q[st]);
       const uint64_t dob_desc = gmma_desc(qmn, sm.dout[st]);
       wgmma_fence();
@@ -621,45 +642,82 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
         const uint32_t a4[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
         wgmma_rs<BF16, D, 1>(dv, a4, gmma_desc_add(dob_desc, kk * 2048), 1u);
       }
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint32_t a4[4] = {da[4 * kk], da[4 * kk + 1], da[4 * kk + 2], da[4 * kk + 3]};
-        wgmma_rs<BF16, D, 1>(dk, a4, gmma_desc_add(qb_desc, kk * 2048), 1u);
-      }
-      wgmma_commit();
       if constexpr (ONE_PASS) {
-        // dQ[q][d] (+)= dS[q][key] K[key][d] over this warpgroup's 64 keys, 64 columns of d at a time
-        const int bh = it.b * p.heads + t.rep * p.kv_heads + it.kvh;
-        const uint64_t a_desc = gmma_desc(dsmn, sm.ds[W]);
-#pragma unroll 1
-        for (int dh = 0; dh < D / 64; ++dh) {
-          float dq[32];
-          const uint64_t b_desc = gmma_desc(kmn, sm.k + W * SUB64 + dh * SUB128);
-          wgmma_fence();
+        wgmma_commit();
+        // dS^T -> this warpgroup's 64 key rows of the shared [128 keys][64 queries] tile (128B swizzle): the K-major A
+        // of dK += dS^T Q and, read MN-major, the A of dQ = dS K.
+        uint8_t* ds = sm.ds[n_ds & 1];
+        ++n_ds;
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            wgmma_ss<BF16, 64, 1, 1>(dq, gmma_desc_add(a_desc, kk * 2048), gmma_desc_add(b_desc, kk * 2048),
-                                     kk > 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<0>();
-          fence_regs(dq);
+        for (int i = 0; i < 16; ++i) {
+          const int row = 64 * W + r_lo + 8 * (i & 1);
+          const int col = 8 * (i / 2) + cq;
+          *reinterpret_cast<uint32_t*>(ds + sw128_off(row, col)) = da[i];
+        }
+        fence_proxy_async_shared();
+        // the previous tile's bulk reduce has finished reading the staging buffer before anyone passes the barrier
+        if (wg_tid == 0) bulk_wait_read<0>();
+        named_bar_sync(1, 256);  // both halves of dS^T are in place
+        const uint64_t dsk_desc = gmma_desc(KMAJ, ds + W * SUB64);
+        const uint64_t dsq_desc = gmma_desc(dsmn, ds);
+        const uint64_t kb_desc = gmma_desc(kmn, sm.k + W * SUB128);
+        float dq[32];
+        wgmma_fence();
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float* drow = p.dq_acc + ((size_t)bh * p.n_pad + c0 + r_lo + 8 * h) * D + dh * 64;
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<BF16, D, 0, 1>(dk, gmma_desc_add(dsk_desc, kk * 32), gmma_desc_add(qb_desc, kk * 2048), 1u);
+        // dQ[64 q][64 W ..] = dS[q][128 keys] K[128 keys][64 W ..]
 #pragma unroll
-            for (int j = 0; j < 8; ++j) red_add_v2(drow + 8 * j + cq, dq[4 * j + 2 * h], dq[4 * j + 2 * h + 1]);
+        for (int kk = 0; kk < 8; ++kk)
+          wgmma_ss<BF16, 64, 1, 1>(dq, gmma_desc_add(dsq_desc, kk * 2048), gmma_desc_add(kb_desc, kk * 2048),
+                                   kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dv);
+        fence_regs(dk);
+        fence_regs(dq);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sm.qd_empty[st]);
+
+        // stage dQ in the layout of map_dq's 128B-swizzled [64 rows][32 fp32] box, then two tensor reductions add it
+        // into dq_acc (rows past n_q carry exact zeros and stay inside n_pad, a multiple of 64)
+        float* stage = sm.dq_stage[W];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r_lo + 8 * h;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int chunk = 2 * (j % 4) + cq / 4;  // 16-byte chunk of the 128-byte box row
+            *reinterpret_cast<float2*>(stage + (j / 4) * 2048 + row * 32 + ((chunk ^ (row & 7)) * 4) + cq % 4) =
+                make_float2(dq[4 * j + 2 * h], dq[4 * j + 2 * h + 1]);
           }
         }
-        named_bar_sync(1 + W, 128);  // every warp is done reading dS^T before it is overwritten
+        fence_proxy_async_shared();
+        named_bar_sync(2 + W, 128);
+        if (wg_tid == 0) {
+          const int bh = it.b * p.heads + t.rep * p.kv_heads + it.kvh;
+          tma_reduce_add_2d(map_dq, stage, 64 * W, bh * p.n_pad + c0);
+          tma_reduce_add_2d(map_dq, stage + 2048, 64 * W + 32, bh * p.n_pad + c0);
+          bulk_commit();
+        }
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint32_t a4[4] = {da[4 * kk], da[4 * kk + 1], da[4 * kk + 2], da[4 * kk + 3]};
+          wgmma_rs<BF16, D, 1>(dk, a4, gmma_desc_add(qb_desc, kk * 2048), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dv);
+        fence_regs(dk);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sm.qd_empty[st]);
       }
-      wgmma_wait<0>();
-      fence_regs(dv);
-      fence_regs(dk);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.qd_empty[st]);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm.kv_empty);
+    // the item's dQ reductions are complete before the CTA can exit (and its shared memory go away)
+    if (ONE_PASS && wg_tid == 0) bulk_wait<0>();
 
     // epilogue: dK carries the folded softmax scale
     bool ring = false;
@@ -702,7 +760,7 @@ __device__ __forceinline__ void dkv_consumer(DkvSmem<D>& sm, const P& p, const i
 template <int D, bool BF16, bool ONE_PASS, bool DOCS, class P>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap map_qd64, const __grid_constant__ CUtensorMap map_kv,
-                    const __grid_constant__ P p) {
+                    const __grid_constant__ CUtensorMap map_dq, const __grid_constant__ P p) {
   extern __shared__ uint8_t smem_raw[];
   DkvSmem<D>& sm = *reinterpret_cast<DkvSmem<D>*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x / 32;
@@ -716,12 +774,14 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap map_qd64, const __grid_c
     fence_mbar_init();
   }
   __syncthreads();
+  // one-pass: the asynchronous consumer schedule spills less at 240 registers than at 232 (232 against 380 bytes of
+  // spill stores, CUDA 12.9); the producer warp's own spills at 24 stay off the consumers' path
   if (warp >= 8) {
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<ONE_PASS ? 24 : 40>();
     if (warp == 8) dkv_producer<D, ONE_PASS, DOCS>(sm, p, &map_qd64, &map_kv);
   } else {
-    setmaxnreg_inc<232>();
-    dkv_consumer<D, BF16, ONE_PASS, DOCS>(sm, p, warp < 4 ? 0 : 1);
+    setmaxnreg_inc<ONE_PASS ? 240 : 232>();
+    dkv_consumer<D, BF16, ONE_PASS, DOCS>(sm, p, &map_dq, warp < 4 ? 0 : 1);
   }
 }
 
@@ -855,7 +915,7 @@ void launch_attn_bwd_dq(const CUtensorMap& map_qd, const CUtensorMap& map_kv, co
 template <int D>
 void launch_attn_bwd_dkdv(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdParams& p,
                           int num_sms, cudaStream_t stream) {
-  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnBwdParams);
+  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnBwdParams);
   Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_bwd_dkv_kernel<D, true, false, true, AttnBwdParams>
                                                    : attn_bwd_dkv_kernel<D, false, false, true, AttnBwdParams>)
                                      : (p.is_bf16 ? attn_bwd_dkv_kernel<D, true, false, false, AttnBwdParams>
@@ -865,13 +925,13 @@ void launch_attn_bwd_dkdv(const CUtensorMap& map_qd64, const CUtensorMap& map_kv
              "bwd_dkdv smem attr");
   const int items = p.batch * p.kv_heads * ((p.n_k + 127) / 128);
   const int grid = items < num_sms ? items : num_sms;
-  void* args[] = {(void*)&map_qd64, (void*)&map_kv, (void*)&p};
+  void* args[] = {(void*)&map_qd64, (void*)&map_kv, (void*)&map_kv /* map_dq: one-pass form only */, (void*)&p};
   cuda_check(cudaLaunchKernel((void*)kern, dim3(grid), dim3(NTHREADS), args, smem, stream), "bwd_dkdv launch");
 }
 
-void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdFusedParams& p,
-                           int num_sms, cudaStream_t stream) {
-  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const AttnBwdFusedParams);
+void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const CUtensorMap& map_dq,
+                           const AttnBwdFusedParams& p, int num_sms, cudaStream_t stream) {
+  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnBwdFusedParams);
   Kern kern = p.doc_spans != nullptr ? (p.is_bf16 ? attn_bwd_dkv_kernel<128, true, true, true, AttnBwdFusedParams>
                                                    : attn_bwd_dkv_kernel<128, false, true, true, AttnBwdFusedParams>)
                                      : (p.is_bf16 ? attn_bwd_dkv_kernel<128, true, true, false, AttnBwdFusedParams>
@@ -880,7 +940,7 @@ void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_k
   cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "bwd_fused smem attr");
   const int items = p.hop_count * p.batch * p.kv_heads * ((p.n_k + 127) / 128);
   const int grid = items < num_sms ? items : num_sms;
-  void* args[] = {(void*)&map_qd64, (void*)&map_kv, (void*)&p};
+  void* args[] = {(void*)&map_qd64, (void*)&map_kv, (void*)&map_dq, (void*)&p};
   cuda_check(cudaLaunchKernel((void*)kern, dim3(grid), dim3(NTHREADS), args, smem, stream), "bwd_fused launch");
 }
 

@@ -528,6 +528,11 @@ std::tuple<Tensor, Tensor> attn_bwd_ring(const Tensor& qdo, const Tensor& kv_buf
                            (hop_mode ? (size_t)slot_owner * kstr[2] * 2 : 0);  // see attn_fwd_impl
   CUtensorMap map_kv = rab::make_tmap_bf16(kv_base, 4, kdims, kstr, kbox, rab::TmapSwizzle::B128);
   p.dq_acc = dq_acc.data_ptr<float>();
+  // dq_acc as rows (b*h*n_pad) of d fp32: one 64-query x 32-column box per tensor reduction
+  uint64_t ddims[2] = {(uint64_t)d, (uint64_t)batch * heads * n_pad};
+  uint64_t dstr[1] = {(uint64_t)d * 4};
+  uint32_t dbox[2] = {32, 64};
+  CUtensorMap map_dq = rab::make_tmap_f32(p.dq_acc, 2, ddims, dstr, dbox, rab::TmapSwizzle::B128);
 
   Tensor dk, dv;
   if (dkv_acc_ptrs.empty()) {
@@ -543,7 +548,7 @@ std::tuple<Tensor, Tensor> attn_bwd_ring(const Tensor& qdo, const Tensor& kv_buf
     p.ring_reduce = 1;
     for (int o = 0; o < world; ++o) p.dkv_acc[o] = reinterpret_cast<float*>(dkv_acc_ptrs[o]);
   }
-  rab::launch_attn_bwd_fused(map_qd64, map_kv, p, sm_count(), stream);
+  rab::launch_attn_bwd_fused(map_qd64, map_kv, map_dq, p, sm_count(), stream);
   return {dk, dv};
 }
 

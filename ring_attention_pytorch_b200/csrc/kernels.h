@@ -147,8 +147,9 @@ struct AttnBwdFusedParams {
   float* dkv_acc[kMaxWorld];
   const int* doc_spans;      // [world][batch][n][2] document intervals, null = off (see AttnFwdParams)
 };
-void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const AttnBwdFusedParams& p,
-                           int num_sms, cudaStream_t stream);
+// map_dq: fp32 map over dq_acc [b*h*n_pad][d], box (32, 64), 128B swizzle (target of the dQ tensor reductions)
+void launch_attn_bwd_fused(const CUtensorMap& map_qd64, const CUtensorMap& map_kv, const CUtensorMap& map_dq,
+                           const AttnBwdFusedParams& p, int num_sms, cudaStream_t stream);
 size_t attn_bwd_fused_smem_bytes();
 // fp32 accumulator [b*h][n_pad][d] -> 16 bit [b][n][h][d], multiplied by scale
 void launch_acc_convert(const float* acc, void* out, int batch, int heads, int n, int n_pad, int d, float scale,

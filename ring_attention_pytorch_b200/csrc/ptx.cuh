@@ -93,8 +93,8 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
 }
 // Watchdog report: the block and call-site tag of the watchdog that fired are left in rab_watchdog_info (and printed
 // when RAB_WATCHDOG_PRINTF is 1), then the kernel traps.  printf is a function call, and a call anywhere in a kernel
-// makes ptxas serialize its wgmma (C7510).  The attention kernels keep it: with the serialized schedule they measured
-// faster on H100 (ptxas spills more in the unserialized one).  The decode kernel defines RAB_WATCHDOG_PRINTF 0.
+// makes ptxas serialize its wgmma (C7510).  The backward (attn_bwd_sm90.cu) and tensor-core decode translation units
+// define RAB_WATCHDOG_PRINTF 0; the forward still keeps the printf.
 #ifndef RAB_WATCHDOG_PRINTF
 #define RAB_WATCHDOG_PRINTF 1
 #endif
@@ -181,6 +181,13 @@ __device__ __forceinline__ void bulk_reduce_add_f32(void* gdst, const void* smem
   asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(gdst),
                "r"(smem_u32(smem_src)), "r"(bytes)
                : "memory");
+}
+// Tensor reduce-add shared -> global (fp32 map, .add), tracked by the issuing thread's bulk async-group.
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
+  asm volatile(
+      "cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
+      "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+      : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
