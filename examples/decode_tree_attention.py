@@ -17,6 +17,9 @@ tokens are appended round-robin so that the shards stay balanced.
 
     # ragged batch (seeded prompt lengths in [0, context]) and a look-back window of 4096 tokens
     ... examples/decode_tree_attention.py --context 1048576 --batch 16 --ragged --window 4096
+
+    # speculative verification: every step appends 4 draft tokens and checks them in one decode call
+    ... examples/decode_tree_attention.py --context 1048576 --batch 16 --draft 4
 """
 from __future__ import annotations
 
@@ -45,6 +48,8 @@ def parse_args(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--ragged", action="store_true", help="per-sequence prompt lengths drawn from the seed in [0, context]")
     ap.add_argument("--window", type=int, default=None, help="look-back window: the query sees positions >= pos - W")
+    ap.add_argument("--draft", type=int, default=1,
+                    help="query tokens per step: append M tokens and decode them in one call (causal among themselves)")
     return ap.parse_args(argv)
 
 
@@ -68,7 +73,7 @@ class ShardedKVCache:
 
 def run(args) -> float:
     """Inside an initialised process group.  Returns the largest error seen with ``--check`` (0.0 otherwise)."""
-    if args.ragged or args.window is not None:
+    if args.ragged or args.window is not None or args.draft > 1:
         return run_ragged(args)
     from ring_attention_pytorch_b200 import tree_attn_decode
 
@@ -154,9 +159,10 @@ def run(args) -> float:
 
 
 def run_ragged(args) -> float:
-    """``--ragged`` / ``--window``: every sequence has its own length, the decode passes the whole capacity buffers with
-    per-sequence ``cache_seqlens``, query positions and ``kv_pos = (rank, world)`` (token t of a sequence lives on rank
-    t % world at local slot t // world).  Slots past a sequence's length hold NaN (0x7F in e4m3): they must not matter."""
+    """``--ragged`` / ``--window`` / ``--draft``: every sequence has its own length, the decode passes the whole capacity
+    buffers with per-sequence ``cache_seqlens``, query positions and ``kv_pos = (rank, world)`` (token t of a sequence
+    lives on rank t % world at local slot t // world).  Slots past a sequence's length hold NaN (0x7F in e4m3): they
+    must not matter.  Each step appends ``--draft`` tokens and decodes all of them in one call."""
     from ring_attention_pytorch_b200 import tree_attn_decode
     from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
     from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda
@@ -165,7 +171,7 @@ def run_ragged(args) -> float:
     cuda = args.device == "cuda"
     dev = torch.device("cuda", torch.cuda.current_device()) if cuda else torch.device("cpu")
     dt = torch.bfloat16 if cuda else torch.float32
-    b, h, hk, d = args.batch, args.heads, args.kv_heads, args.dim_head
+    b, h, hk, d, M = args.batch, args.heads, args.kv_heads, args.dim_head, args.draft
     assert not (args.fp8 and not cuda), "the fp8 cache needs the sm_90a kernel"
     gen = torch.Generator().manual_seed(args.seed)  # the same on every rank: lengths, queries, new tokens
     lens = torch.full((b,), args.context, dtype=torch.int64)
@@ -177,7 +183,7 @@ def run_ragged(args) -> float:
     def local_len(n):  # tokens rank, rank + world, ... below n
         return (n - rank + world - 1).clamp(min=0) // world
 
-    cap = (args.context + args.steps + world - 1) // world + 1
+    cap = (args.context + args.steps * M + world - 1) // world + 1
     n0 = (args.context + world - 1) // world
     dgen = torch.Generator(device=dev).manual_seed(args.seed * 7919 + 1 + rank)
     pk = torch.randn(b, hk, n0, d, generator=dgen, device=dev)
@@ -205,7 +211,7 @@ def run_ragged(args) -> float:
 
     full_k = full_v = None
     if args.check:  # global [b, hk, max length, d] in position order, from every rank's slots
-        total = int(lens.max()) + args.steps
+        total = int(lens.max()) + args.steps * M
         full_k, full_v = torch.zeros(b, hk, total, d), torch.zeros(b, hk, total, d)
         parts = [None] * world
         dist.all_gather_object(parts, (quantised(kc.float(), k_scale).cpu(), quantised(vc.float(), v_scale).cpu()))
@@ -216,20 +222,22 @@ def run_ragged(args) -> float:
 
     worst, times, seen = 0.0, [], 0
     for _ in range(args.steps):
-        q = torch.randn(b, h, 1, d, generator=gen).to(dev, dt)
-        k_new, v_new = torch.randn(b, hk, d, generator=gen), torch.randn(b, hk, d, generator=gen)
+        q = torch.randn(b, h, M, d, generator=gen).to(dev, dt)
+        k_new, v_new = torch.randn(b, hk, M, d, generator=gen), torch.randn(b, hk, M, d, generator=gen)
         if args.fp8:
-            k_new, v_new = k_new / k_scale.view(b, hk, 1).cpu(), v_new / v_scale.view(b, hk, 1).cpu()
-        mine = (lens % world == rank).nonzero().flatten()  # the new token of sequence i goes to rank lens[i] % world
-        slot = held[mine]
-        kc[mine.to(dev), :, slot.to(dev)] = k_new[mine].to(dev, cache_dtype)
-        vc[mine.to(dev), :, slot.to(dev)] = v_new[mine].to(dev, cache_dtype)
-        q_pos = lens.clone()  # the new token's position
-        lens += 1
+            k_new, v_new = k_new / k_scale.view(b, hk, 1, 1).cpu(), v_new / v_scale.view(b, hk, 1, 1).cpu()
+        for u in range(M):  # new token u of sequence i sits at lens[i] + u and goes to rank (lens[i] + u) % world
+            pos = lens + u
+            mine = (pos % world == rank).nonzero().flatten()
+            slot = local_len(pos)[mine]
+            kc[mine.to(dev), :, slot.to(dev)] = k_new[mine, :, u].to(dev, cache_dtype)
+            vc[mine.to(dev), :, slot.to(dev)] = v_new[mine, :, u].to(dev, cache_dtype)
+        q_pos = lens.clone()  # the first new token's position
+        lens += M
         held = local_len(lens)
         kw = dict(cache_seqlens=held.to(dev, torch.int32), q_pos=q_pos.to(dev, torch.int32), window=args.window,
                   kv_pos=(rank, world))
-        seen += int(sum(min(int(n), (args.window or int(n)) + 1) for n in lens))
+        seen += int(sum(min(int(n), (args.window or int(n)) + M) for n in lens))
         if cuda:
             torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
@@ -241,21 +249,23 @@ def run_ragged(args) -> float:
             torch.cuda.synchronize(dev)
         times.append(time.perf_counter() - t0)
         if args.check:
-            kq = quantised(k_new[:, :, None], k_scale.cpu() if k_scale is not None else None)[:, :, 0]
-            vq = quantised(v_new[:, :, None], v_scale.cpu() if v_scale is not None else None)[:, :, 0]
+            kq = quantised(k_new, k_scale.cpu() if k_scale is not None else None)
+            vq = quantised(v_new, v_scale.cpu() if v_scale is not None else None)
             for i in range(b):
-                full_k[i, :, q_pos[i]], full_v[i, :, q_pos[i]] = kq[i], vq[i]
+                p0 = int(q_pos[i])
+                full_k[i, :, p0:p0 + M], full_v[i, :, p0:p0 + M] = kq[i], vq[i]
                 n = int(lens[i])
                 ref = attention_with_positions(q[i:i + 1].float().cpu().transpose(1, 2),
                                                full_k[i:i + 1, :, :n].transpose(1, 2), full_v[i:i + 1, :, :n].transpose(1, 2),
-                                               q_pos=q_pos[i:i + 1], k_pos=torch.arange(n), causal=True, window=args.window)
+                                               q_pos=p0 + torch.arange(M), k_pos=torch.arange(n), causal=True,
+                                               window=args.window)
                 worst = max(worst, float((out[i:i + 1].float().cpu() - ref.transpose(1, 2)).abs().max()))
     if rank == 0:
         ts = sorted(times[min(3, len(times) - 1):])
         med = ts[len(ts) // 2]
         kv_bytes = 2 * hk * d * (seen / args.steps) * (1 if args.fp8 else (2 if cuda else 4))
-        print(f"[decode] world {world}, ragged {args.ragged}, window {args.window}, lengths {int(lens.min())}.."
-              f"{int(lens.max())}, batch {b}, heads {h}/{hk}: median step {med * 1e3:.3f} ms, {b / med:.0f} tokens/s, "
+        print(f"[decode] world {world}, ragged {args.ragged}, window {args.window}, draft {M}, lengths {int(lens.min())}.."
+              f"{int(lens.max())}, batch {b}, heads {h}/{hk}: median step {med * 1e3:.3f} ms, {b * M / med:.0f} tokens/s, "
               f"visible cache read {kv_bytes / med / 1e9:.0f} GB/s whole job"
               + (f", max |err| vs dense {worst:.2e}" if args.check else ""), flush=True)
     return worst

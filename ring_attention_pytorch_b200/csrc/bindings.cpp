@@ -569,9 +569,10 @@ void acc_convert(const Tensor& acc, Tensor out, double scale) {
 // cross-rank signal, merge over NVLink loads or NVLS multimem reductions).  Every buffer is owned by the caller
 // (ops/tree_decode_cuda.py caches them), so the call allocates nothing and can be captured in a CUDA graph.
 // ---------------------------------------------------------------------------------------------
-int64_t tree_decode_max_ctas(int64_t d, int64_t kv_kind, bool tensor_core, bool ranged) {
-  if (tensor_core) return rab::tree_decode_tc_max_ctas((int)kv_kind, sm_count(), ranged);
-  return rab::tree_decode_max_ctas((int)d, (int)kv_kind, sm_count(), ranged);
+// cols > 0: a multi-token call with g * tokens (query head, token) columns per kv head
+int64_t tree_decode_max_ctas(int64_t d, int64_t kv_kind, bool tensor_core, bool ranged, int64_t cols) {
+  if (tensor_core) return rab::tree_decode_tc_max_ctas((int)kv_kind, sm_count(), ranged, (int)cols);
+  return rab::tree_decode_max_ctas((int)d, (int)kv_kind, sm_count(), ranged, cols > 0);
 }
 
 // int32 [b] on q's device (ranged decode: per-sequence cache lengths / query positions), or null
@@ -591,8 +592,11 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
                  bool tensor_core, const c10::optional<Tensor>& sinks, const c10::optional<Tensor>& cache_seqlens,
                  const c10::optional<Tensor>& q_pos, int64_t window, int64_t kv_pos_offset, int64_t kv_pos_stride,
                  double softclamp) {
-  TORCH_CHECK(q.is_cuda() && q.is_contiguous() && q.dim() == 3, "q must be contiguous [b, h, d]");
-  const int b = q.size(0), h = q.size(1), d = q.size(2);
+  TORCH_CHECK(q.is_cuda() && q.is_contiguous() && (q.dim() == 3 || q.dim() == 4),
+              "q must be contiguous [b, h, d] or [b, h, tokens, d]");
+  const int b = q.size(0), h = q.size(1), d = q.size(-1);
+  const int tokens = q.dim() == 4 ? (int)q.size(2) : 1;
+  TORCH_CHECK(tokens >= 1, "q needs at least one token");
   TORCH_CHECK(d == 64 || d == 128, "tree decode supports head dim 64 or 128");
   rab::TreeDecodeParams p;
   std::memset(&p, 0, sizeof(p));
@@ -641,10 +645,11 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   p.batch = b; p.heads = h; p.kv_heads = (int)kv_heads; p.n = n; p.splits = (int)splits;
   TORCH_CHECK(h % kv_heads == 0 && splits >= 1);
   p.scale_log2 = (float)(scale * 1.4426950408889634);
-  const int g = h / (int)kv_heads;
+  const int g = h / (int)kv_heads * tokens;  // columns per kv head
   TORCH_CHECK(scratch.scalar_type() == at::kFloat && scratch.is_contiguous() &&
               scratch.numel() >= (int64_t)b * kv_heads * splits * g * (d + 4));
   TORCH_CHECK(group_done.scalar_type() == at::kInt && group_done.numel() >= (int64_t)b * kv_heads * ((g + 3) / 4));
+  p.tokens = tokens;
   TORCH_CHECK(counters.scalar_type() == at::kInt && counters.numel() >= 4);
   p.scratch = scratch.data_ptr<float>();
   p.group_done = reinterpret_cast<uint32_t*>(group_done.data_ptr<int>());
@@ -660,7 +665,7 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   p.aux_local = reinterpret_cast<float*>(aux_local_ptr);
   p.mc_partial = reinterpret_cast<const float*>(mc_partial_ptr);
   p.mc_aux = reinterpret_cast<const float*>(mc_aux_ptr);
-  TORCH_CHECK(out.is_cuda() && out.is_contiguous() && out.numel() == (int64_t)b * h * d);
+  TORCH_CHECK(out.is_cuda() && out.is_contiguous() && out.numel() == (int64_t)b * h * tokens * d);
   p.out = out.data_ptr();
   p.out_kind = out.scalar_type() == at::kBFloat16 ? 1 : (out.scalar_type() == at::kHalf ? 0 : 2);
   TORCH_CHECK(p.out_kind != 2 || out.scalar_type() == at::kFloat);
@@ -677,7 +682,8 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   p.kv_pos_offset = (int)kv_pos_offset;
   p.kv_pos_stride = (int)kv_pos_stride;
   p.softclamp_log2 = (float)(softclamp * 1.4426950408889634);
-  const bool ranged = p.cache_seqlens != nullptr || p.q_pos != nullptr || softclamp > 0.0;
+  // a multi-token call always takes the ranged body (its kernels derive per-token key ranges)
+  const bool ranged = p.cache_seqlens != nullptr || p.q_pos != nullptr || softclamp > 0.0 || tokens > 1;
   c10::cuda::CUDAGuard guard(q.device());
   if (tensor_core) {
     TORCH_CHECK(d == 128 && n > 0, "the tensor-core decode kernel needs head dim 128 and a non-empty shard");
@@ -819,7 +825,7 @@ TORCH_LIBRARY(rab, m) {
         "mc_aux_ptr, int rank, Tensor(d!) out, int kv_heads, int splits, float scale, int scale_block_keys, float eps, "
         "int grid, bool tensor_core, Tensor? sinks=None, Tensor? cache_seqlens=None, Tensor? q_pos=None, int window=0, "
         "int kv_pos_offset=0, int kv_pos_stride=1, float softclamp=0.0) -> ()");
-  m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core, bool ranged=False) -> int");
+  m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core, bool ranged=False, int cols=0) -> int");
   m.def("bwd_prep(Tensor q, Tensor o, Tensor dout, Tensor lse, Tensor(a!) qdo_buf, Tensor(b!) stat_buf, int rank, "
         "Tensor? sinks=None, Tensor(c!)? dsinks=None) -> ()");
   m.def("attn_bwd_dq(Tensor qdo_buf, Tensor kv_buf, Tensor stat_buf, Tensor? ready, int ready_target, Tensor? "

@@ -167,7 +167,7 @@ void launch_bwd_prep(const void* q, const void* o, const void* dout, const float
 // tree-attention decode (tree_decode_sm90.cu): ONE persistent cooperative kernel per rank and step
 // ------------------------------------------------------------------------------------------------
 struct TreeDecodeParams {
-  const void* q;            // [b, h, d]; q_kind 0 bf16, 1 fp16, 2 fp32
+  const void* q;            // [b, h, d] ([b, h, tokens, d] multi-token); q_kind 0 bf16, 1 fp16, 2 fp32
   int q_kind;
   const void* k;            // [b*hk, n, d]; kv_kind 0 bf16, 1 fp16, 2 fp8-e4m3
   const void* v;
@@ -204,11 +204,18 @@ struct TreeDecodeParams {
   int window;
   int kv_pos_offset, kv_pos_stride;   // >= 0, >= 1
   float softclamp_log2;               // > 0: logits (log2 units) become c tanh(s / c) with c = softclamp * log2(e)
+  // Multi-token decode (the `multi` instantiations, always ranged; the others read neither field's value): q holds
+  // `tokens` consecutive query tokens per (batch, head), q / out [b, h, tokens, d], partial rows (b, head, token).
+  // Token t sits at q_pos[b] + t (the position rule above per token); the work unit's columns are the g * tokens
+  // (query head, token) pairs of one kv head, column c = (head slot c / tokens, token c % tokens).
+  int tokens;
 };
-int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged);
+int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged, bool multi = false);
+// p.tokens > 1 launches the multi-token instantiations
 void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream, bool ranged);
-// wgmma variant (tree_decode_tc_sm90.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 64-key box
-int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged);
+// wgmma variant (tree_decode_tc_sm90.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 64-key box.
+// cols: (query head, token) columns per kv head of a multi-token call (g * tokens), 0 for a single-token call
+int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged, int cols = 0);
 void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, const TreeDecodeParams& p, int grid,
                            cudaStream_t stream, bool ranged);
 

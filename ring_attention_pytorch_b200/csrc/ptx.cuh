@@ -353,6 +353,32 @@ __device__ __forceinline__ void wgmma_ss_n16(float (&d)[8], uint64_t a_desc, uin
 }
 
 template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma16_ss_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
 __device__ __forceinline__ void wgmma16_ss_n8(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
       "{\n"
@@ -422,13 +448,16 @@ __device__ __forceinline__ void wgmma_e4m3_rs_n64(float (&d)[32], const uint32_t
 
 template <bool BF16, int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
-  static_assert(N == 8 || N == 16 || N == 64 || N == 128, "wgmma N");
+  static_assert(N == 8 || N == 16 || N == 32 || N == 64 || N == 128, "wgmma N");
   if constexpr (N == 8) {
     if constexpr (BF16) wgmma_ss_n8<TA, TB>(d, a_desc, b_desc, scale_d);
     else wgmma16_ss_n8<TA, TB>(d, a_desc, b_desc, scale_d);
   } else if constexpr (N == 16) {
     if constexpr (BF16) wgmma_ss_n16<TA, TB>(d, a_desc, b_desc, scale_d);
     else wgmma16_ss_n16<TA, TB>(d, a_desc, b_desc, scale_d);
+  } else if constexpr (N == 32) {
+    if constexpr (BF16) wgmma_ss_n32<TA, TB>(d, a_desc, b_desc, scale_d);
+    else wgmma16_ss_n32<TA, TB>(d, a_desc, b_desc, scale_d);
   } else if constexpr (N == 64) {
     if constexpr (BF16) wgmma_ss_n64<TA, TB>(d, a_desc, b_desc, scale_d);
     else wgmma16_ss_n64<TA, TB>(d, a_desc, b_desc, scale_d);

@@ -17,23 +17,25 @@ __device__ __forceinline__ float load_q(const void* q, int kind, size_t idx) {
 
 // Ranged decode: the keys unit (b, split) covers, [k0, k1), and the first visible key lo (keys in [k0, lo) are masked).
 // Tiles start at lo rounded down to a multiple of TILE, so they stay aligned with the scale blocks of an fp8 cache.
+// MULTI: the union of the visible ranges of the p.tokens query tokens (lo from the first token, hi from the last).
 struct TdUnitRange {
   int lo, k0, k1;
 };
 __device__ __forceinline__ long long td_floor_div(long long a, long long b) {  // b > 0, any sign of a
   return a >= 0 ? a / b : -((-a + b - 1) / b);
 }
-template <int TILE>
+template <int TILE, bool MULTI = false>
 __device__ __forceinline__ TdUnitRange td_unit_range(const TreeDecodeParams& p, int b, int split) {
   long long lo = 0, hi = p.n;
   if (p.cache_seqlens != nullptr) hi = min(hi, (long long)p.cache_seqlens[b]);
   long long span = p.n;  // the most keys (with tile slack) one sequence's visible range can touch
   if (p.q_pos != nullptr) {
     const long long rel = (long long)p.q_pos[b] - p.kv_pos_offset;  // negative: every key here lies after the query
-    hi = min(hi, td_floor_div(rel, p.kv_pos_stride) + 1);             // P(j) <= q_pos
+    const long long last = MULTI ? (long long)p.tokens - 1 : 0;        // the last token sits at q_pos + last
+    hi = min(hi, td_floor_div(rel + last, p.kv_pos_stride) + 1);      // P(j) <= q_pos (+ last)
     if (p.window > 0) {
       lo = max(lo, -td_floor_div((long long)p.window - rel, p.kv_pos_stride));  // q_pos - P(j) <= window
-      span = min(span, (long long)p.window / p.kv_pos_stride + TILE);
+      span = min(span, ((long long)p.window + last) / p.kv_pos_stride + TILE);
     }
   }
   lo = min(lo, (long long)p.n);
@@ -42,6 +44,23 @@ __device__ __forceinline__ TdUnitRange td_unit_range(const TreeDecodeParams& p, 
   r.lo = (int)lo;
   r.k0 = (int)min((lo & ~(long long)(TILE - 1)) + split * per, (long long)p.n);
   r.k1 = lo < hi ? (int)max(min(hi, (long long)r.k0 + per), (long long)r.k0) : r.k0;
+  return r;
+}
+
+// Multi-token decode: the keys of [lo, k1) (a unit's range) that token t sees, [clo, chi) (empty when chi <= clo).
+struct TdColRange {
+  int lo, hi;
+};
+__device__ __forceinline__ TdColRange td_col_range(const TreeDecodeParams& p, int b, int t, int lo, int k1) {
+  long long clo = lo, chi = k1;
+  if (p.q_pos != nullptr) {
+    const long long rel = (long long)p.q_pos[b] + t - p.kv_pos_offset;
+    chi = min(chi, td_floor_div(rel, p.kv_pos_stride) + 1);
+    if (p.window > 0) clo = max(clo, -td_floor_div((long long)p.window - rel, p.kv_pos_stride));
+  }
+  TdColRange r;
+  r.lo = (int)min(clo, (long long)k1);
+  r.hi = (int)max(chi, (long long)lo);
   return r;
 }
 
@@ -92,8 +111,8 @@ __device__ __forceinline__ void grid_barrier(uint32_t* count, uint32_t* gen) {
 }
 
 // State every thread derives from the launch parameters: which half of the double-buffered symmetric buffers this call
-// uses and the epoch it signals with.
-template <int D>
+// uses and the epoch it signals with.  MULTI: rows are (batch, head, token), b * h * tokens of them.
+template <int D, bool MULTI = false>
 struct TdCall {
   static constexpr int row_stride = D + 4;  // (out[D], lse2, valid, pad, pad): rows stay 16-byte aligned
   uint32_t base;
@@ -107,17 +126,23 @@ struct TdCall {
     base = ld_acquire_gpu(&p.counters[3]);  // block 0 advances it behind the last grid barrier
     const bool nvls_cfg = p.mc_partial != nullptr && p.world > 1;
     const uint32_t call = nvls_cfg ? (base >> 1) : base;
-    half_off = (size_t)(call & 1u) * (size_t)p.batch * p.heads * row_stride;
-    aux_off = (size_t)(call & 1u) * (size_t)p.batch * p.heads * 2;
+    if constexpr (MULTI) {
+      half_off = (size_t)(call & 1u) * (size_t)p.batch * p.heads * p.tokens * row_stride;
+      aux_off = (size_t)(call & 1u) * (size_t)p.batch * p.heads * p.tokens * 2;
+    } else {
+      half_off = (size_t)(call & 1u) * (size_t)p.batch * p.heads * row_stride;
+      aux_off = (size_t)(call & 1u) * (size_t)p.batch * p.heads * 2;
+    }
     my_partial = p.partial_local + half_off;
     my_aux = p.aux_local + aux_off;
   }
 };
 
 // Phases 2 and 3 of a decode step; every thread of every CTA of the (cooperative) grid calls it after its last unit.
-template <int D>
-__device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, const TdCall<D>& cs, int total_units) {
-  constexpr int row_stride = TdCall<D>::row_stride;
+template <int D, bool MULTI = false>
+__device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, const TdCall<D, MULTI>& cs,
+                                                    int total_units) {
+  constexpr int row_stride = TdCall<D, MULTI>::row_stride;
   const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
   const int nthreads = blockDim.x;
   uint32_t* const ctr = p.counters;
@@ -126,7 +151,8 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
   float* const my_partial = cs.my_partial;
   float* const my_aux = cs.my_aux;
   if (total_units == 0) {  // this rank holds no keys: publish empty rows
-    for (int i = blockIdx.x * nthreads + tid; i < p.batch * p.heads; i += gridDim.x * nthreads) {
+    for (int i = blockIdx.x * nthreads + tid; i < (MULTI ? p.batch * p.heads * p.tokens : p.batch * p.heads);
+         i += gridDim.x * nthreads) {
       my_partial[(size_t)i * row_stride + D] = -INFINITY;
       my_partial[(size_t)i * row_stride + D + 1] = 0.f;
     }
@@ -135,7 +161,7 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
   // ====================================== phase 2: everyone's partials are visible ====================================
   __threadfence();
   grid_barrier(&ctr[1], &ctr[2]);
-  const int rows = p.batch * p.heads;
+  const int rows = MULTI ? p.batch * p.heads * p.tokens : p.batch * p.heads;
   const int gwarp = blockIdx.x * (nthreads / 32) + warp, nwarps = gridDim.x * (nthreads / 32);
   const bool nvls = p.mc_partial != nullptr && p.world > 1;
   int* const my_ord = reinterpret_cast<int*>(my_aux);  // [rows] order-preserving integer image of this rank's lse
@@ -178,7 +204,7 @@ __device__ __forceinline__ void td_cross_rank_merge(const TreeDecodeParams& p, c
   };
   const bool own = lane * 4 < D;  // one warp per row; lane c owns columns [4c, 4c + 4)
   // attention sink of row bh in log2 units: one more term of the merged denominator, with a zero value vector
-  auto sink2 = [&](int bh) { return p.sinks[bh % p.heads] * 1.4426950408889634f; };
+  auto sink2 = [&](int bh) { return p.sinks[(MULTI ? bh / p.tokens : bh) % p.heads] * 1.4426950408889634f; };
   if (!nvls) {
     // P2P: every rank reads every peer's row straight over NVLink
     for (int bh = gwarp; bh < rows; bh += nwarps) {

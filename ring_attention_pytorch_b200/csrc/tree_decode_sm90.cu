@@ -83,20 +83,23 @@ struct KvVec<2> {
 
 
 // RANGED: per-sequence visible key ranges and softclamp (TreeDecodeParams).  Key loads are clamped into [lo, k1), so a
-// masked key's probability of 0 always multiplies a visible (finite) value row.
-template <int D, int KV_KIND, bool RANGED>
+// masked key's probability of 0 always multiplies a visible (finite) value row.  MULTI (with RANGED): the 4 columns of a
+// unit are (query head, token) pairs of a multi-token call; the unit streams the union of its tokens' key ranges and
+// masks each column with its own token's range.
+template <int D, int KV_KIND, bool RANGED, bool MULTI = false>
 __global__ void __launch_bounds__(TD_THREADS)
 tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
+  static_assert(RANGED || !MULTI, "a multi-token call takes the ranged body");
   using Vec = KvVec<KV_KIND>;
   using Raw = typename Vec::Raw;
   const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
-  const int g_total = p.heads / p.kv_heads;
+  const int g_total = MULTI ? p.heads / p.kv_heads * p.tokens : p.heads / p.kv_heads;  // columns per kv head
   const int zchunks = (g_total + TD_MAX_G - 1) / TD_MAX_G;
   const int groups = p.batch * p.kv_heads * zchunks;       // units = groups x splits
   const int total_units = p.n > 0 ? groups * p.splits : 0;
-  constexpr int row_stride = TdCall<D>::row_stride;
+  constexpr int row_stride = TdCall<D, MULTI>::row_stride;
   uint32_t* const ctr = p.counters;                         // [0] queue head, [1] barrier count, [2] barrier gen, [3] epoch
-  TdCall<D> cs;
+  TdCall<D, MULTI> cs;
   cs.init(p);
   float* const my_partial = cs.my_partial;
 
@@ -132,10 +135,24 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     const int per = ((p.n + p.splits - 1) / p.splits + TD_TILE - 1) / TD_TILE * TD_TILE;  // tile-aligned splits
     int k0 = split * per, k1 = min(p.n, k0 + per), lo = 0;
     if constexpr (RANGED) {
-      const TdUnitRange r = td_unit_range<TD_TILE>(p, b, split);
+      const TdUnitRange r = td_unit_range<TD_TILE, MULTI>(p, b, split);
       k0 = r.k0;
       k1 = r.k1;
       lo = r.lo;
+    }
+    // the partial row of column gi: (b, query head, token)
+    auto prow = [&](int gi) -> size_t {
+      const int c = g0 + gi;
+      return ((size_t)b * p.heads + (size_t)(c / p.tokens) * p.kv_heads + kvh) * p.tokens + c % p.tokens;
+    };
+    int clo[TD_MAX_G], chi[TD_MAX_G];  // multi-token: the keys each column's token sees (read by MULTI only)
+    if constexpr (MULTI) {
+#pragma unroll
+      for (int gi = 0; gi < TD_MAX_G; ++gi) {
+        const TdColRange cr = td_col_range(p, b, (g0 + gi) % p.tokens, lo, k1);
+        clo[gi] = cr.lo;
+        chi[gi] = gi < g ? cr.hi : cr.lo;
+      }
     }
     const float clamp_inv = RANGED && p.softclamp_log2 > 0.f ? 1.f / p.softclamp_log2 : 0.f;
 
@@ -151,7 +168,8 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
 #pragma unroll
       for (int e = 0; e < EPL / 2; ++e) {
         // query head j uses kv head j % kv_heads  ->  heads {kvh, kvh + hk, ...}
-        const size_t qi = ((size_t)b * p.heads + (size_t)(g0 + gi) * p.kv_heads + kvh) * D + l8 * EPL + 2 * e;
+        const size_t qi = MULTI ? prow(gi) * D + l8 * EPL + 2 * e
+                                : ((size_t)b * p.heads + (size_t)(g0 + gi) * p.kv_heads + kvh) * D + l8 * EPL + 2 * e;
         qr[gi][e] = gi < g ? make_float2(load_q(p.q, p.q_kind, qi) * p.scale_log2, load_q(p.q, p.q_kind, qi + 1) * p.scale_log2)
                            : make_float2(0.f, 0.f);
       }
@@ -209,7 +227,11 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
           a += __shfl_xor_sync(0xffffffffu, a, 1);
           a += __shfl_xor_sync(0xffffffffu, a, 2);
           a += __shfl_xor_sync(0xffffffffu, a, 4);
-          if constexpr (RANGED) {
+          if constexpr (MULTI) {
+            float x = a * ks;
+            if (p.softclamp_log2 > 0.f) x = fast_tanh(x * clamp_inv) * p.softclamp_log2;
+            part[gi] = (t0 + kl >= clo[gi] && t0 + kl < chi[gi]) ? x : -INFINITY;
+          } else if constexpr (RANGED) {
             float x = a * ks;
             if (p.softclamp_log2 > 0.f) x = fast_tanh(x * clamp_inv) * p.softclamp_log2;
             part[gi] = live ? x : -INFINITY;
@@ -304,7 +326,7 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
       if (warp < g && lane == 0) {
         corr_s[0][warp] = l_run > 0.f ? 1.f / l_run : 0.f;
         const int head = (g0 + warp) * p.kv_heads + kvh;
-        float* row = my_partial + ((size_t)b * p.heads + head) * row_stride;
+        float* row = my_partial + (MULTI ? prow(warp) : (size_t)b * p.heads + head) * row_stride;
         row[D] = l_run > 0.f ? (m_run == -INFINITY ? 0.f : m_run) + log2f(l_run) : -INFINITY;
         row[D + 1] = l_run > 0.f ? 1.f : 0.f;
       }
@@ -315,7 +337,7 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
 #pragma unroll
         for (int kg = 0; kg < 8; ++kg) sacc += red_s[kg][gi][c];
         const int head = (g0 + gi) * p.kv_heads + kvh;
-        my_partial[((size_t)b * p.heads + head) * row_stride + c] = sacc * corr_s[0][gi];
+        my_partial[(MULTI ? prow(gi) : (size_t)b * p.heads + head) * row_stride + c] = sacc * corr_s[0][gi];
       }
     } else {
       float* out = p.scratch + (((size_t)bhk * p.splits + split) * g_total + g0) * row_stride;
@@ -353,7 +375,7 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
             l += ms == -INFINITY ? 0.f : __ldcg(&base[s * stride + D + 1]) * fast_exp2(ms - m_eff);
           }
           const int head = (g0 + gi) * p.kv_heads + kvh;
-          float* row = my_partial + ((size_t)b * p.heads + head) * row_stride;
+          float* row = my_partial + (MULTI ? prow(gi) : (size_t)b * p.heads + head) * row_stride;
           for (int c = tid; c < D; c += TD_THREADS) {
             float a = 0.f;
             for (int s = 0; s < p.splits; ++s) {
@@ -371,32 +393,34 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     }
     __syncthreads();
   }
-  td_cross_rank_merge<D>(p, cs, total_units);
+  td_cross_rank_merge<D, MULTI>(p, cs, total_units);
 }
 
-template <bool RANGED>
+template <bool RANGED, bool MULTI = false>
 const void* pick_td(int d, int kv_kind) {
   if (d == 128) {
-    if (kv_kind == 0) return (const void*)tree_decode_kernel<128, 0, RANGED>;
-    if (kv_kind == 1) return (const void*)tree_decode_kernel<128, 1, RANGED>;
-    return (const void*)tree_decode_kernel<128, 2, RANGED>;
+    if (kv_kind == 0) return (const void*)tree_decode_kernel<128, 0, RANGED, MULTI>;
+    if (kv_kind == 1) return (const void*)tree_decode_kernel<128, 1, RANGED, MULTI>;
+    return (const void*)tree_decode_kernel<128, 2, RANGED, MULTI>;
   }
-  if (kv_kind == 0) return (const void*)tree_decode_kernel<64, 0, RANGED>;
-  if (kv_kind == 1) return (const void*)tree_decode_kernel<64, 1, RANGED>;
-  return (const void*)tree_decode_kernel<64, 2, RANGED>;
+  if (kv_kind == 0) return (const void*)tree_decode_kernel<64, 0, RANGED, MULTI>;
+  if (kv_kind == 1) return (const void*)tree_decode_kernel<64, 1, RANGED, MULTI>;
+  return (const void*)tree_decode_kernel<64, 2, RANGED, MULTI>;
 }
 
 }  // namespace
 
-int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged) {
+int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged, bool multi) {
   int per_sm = 0;
-  const void* fn = ranged ? pick_td<true>(d, kv_kind) : pick_td<false>(d, kv_kind);
+  const void* fn = multi ? pick_td<true, true>(d, kv_kind)
+                         : (ranged ? pick_td<true>(d, kv_kind) : pick_td<false>(d, kv_kind));
   cuda_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, TD_THREADS, 0), "tree_decode occupancy");
   return per_sm * num_sms;
 }
 
 void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream, bool ranged) {
-  const void* fn = ranged ? pick_td<true>(d, p.kv_kind) : pick_td<false>(d, p.kv_kind);
+  const void* fn = p.tokens > 1 ? pick_td<true, true>(d, p.kv_kind)
+                                : (ranged ? pick_td<true>(d, p.kv_kind) : pick_td<false>(d, p.kv_kind));
   void* args[] = {(void*)&p};
   // cooperative: the grid barrier and the cross-rank waits need every CTA of the grid to be resident
   cuda_check(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(TD_THREADS), args, 0, stream), "tree_decode launch");

@@ -1,4 +1,5 @@
-// Tree-attention decode on the Hopper tensor cores (head dim 128, up to 16 query heads per work unit).
+// Tree-attention decode on the Hopper tensor cores (head dim 128, up to 16 query heads -- or 32 (query head, token)
+// columns of a multi-token call -- per work unit).
 //
 // A decode step is bandwidth bound, but with grouped-query heads the CUDA-core split-KV kernel (tree_decode_sm90.cu)
 // spends g FMAs per loaded element on its own dependency chains.  Here both products run as wgmma in the TRANSPOSED
@@ -19,6 +20,8 @@
 // Reference: tree_attn_decoding.py:60-102.
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
+
+#include <type_traits>
 
 // no printf in the watchdogs: a function call would serialize this kernel's wgmma (see ptx.cuh)
 #define RAB_WATCHDOG_PRINTF 0
@@ -48,6 +51,11 @@ struct TcSmem {
   uint64_t full[TC_NST];
   int unit;
   uint32_t last;
+};
+// multi-token units: the visible keys [clo, chi) of each column (its token's range within the unit's [lo, k1))
+template <bool KV8, int NH>
+struct TcSmemMulti : TcSmem<KV8, NH> {
+  int clo[NH], chi[NH];
 };
 
 template <bool F16>
@@ -83,28 +91,31 @@ __device__ __forceinline__ void widen_fp8_tile(const uint8_t* src, uint8_t* dst,
 
 // KVK: 0 bf16, 1 fp16, 2 fp8-e4m3 cache.  NH: query heads per unit (MMA N).  RANGED: per-sequence visible key ranges
 // and softclamp (TreeDecodeParams); V rows of invisible keys in a unit's boundary tiles are zeroed in shared memory,
-// since a probability of 0 does not cancel a NaN value row inside the MMA.
-template <int KVK, int NH, bool RANGED>
+// since a probability of 0 does not cancel a NaN value row inside the MMA.  MULTI (with RANGED): the columns are the
+// (query head, token) pairs of a multi-token call; the unit streams the union of its tokens' key ranges and, in the
+// tiles that cross some column's bounds, masks each (key, column) with that column's range.
+template <int KVK, int NH, bool RANGED, bool MULTI = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                       const __grid_constant__ TreeDecodeParams p) {
+  static_assert(RANGED || !MULTI, "a multi-token call takes the ranged body");
   constexpr bool KV8 = KVK == 2;
   constexpr bool F16 = KVK == 1;
   constexpr int D = TC_D;
   constexpr int NJ = NH / 8;  // n8 column blocks of the accumulators
-  using Smem = TcSmem<KV8, NH>;
+  using Smem = std::conditional_t<MULTI, TcSmemMulti<KV8, NH>, TcSmem<KV8, NH>>;
   extern __shared__ uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
   const int r_lo = warp * 16 + lane / 4;  // accumulator rows r_lo, r_lo + 8
   const int cq = 2 * (lane % 4);          // accumulator columns 8 j + cq (+1)
-  const int g_total = p.heads / p.kv_heads;
+  const int g_total = MULTI ? p.heads / p.kv_heads * p.tokens : p.heads / p.kv_heads;  // columns per kv head
   const int zchunks = (g_total + NH - 1) / NH;
   const int groups = p.batch * p.kv_heads * zchunks;
   const int total_units = p.n > 0 ? groups * p.splits : 0;
-  constexpr int row_stride = TdCall<D>::row_stride;
+  constexpr int row_stride = TdCall<D, MULTI>::row_stride;
   uint32_t* const ctr = p.counters;
-  TdCall<D> cs;
+  TdCall<D, MULTI> cs;
   cs.init(p);
   float* const my_partial = cs.my_partial;
 
@@ -136,12 +147,40 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
     const int per = ((p.n + p.splits - 1) / p.splits + TC_TILE - 1) / TC_TILE * TC_TILE;  // tile-aligned splits
     int k0 = split * per, k1 = min(p.n, k0 + per), lo = 0;
     if constexpr (RANGED) {
-      const TdUnitRange r = td_unit_range<TC_TILE>(p, b, split);
+      const TdUnitRange r = td_unit_range<TC_TILE, MULTI>(p, b, split);
       k0 = r.k0;
       k1 = r.k1;
       lo = r.lo;
     }
     const int ntiles = k0 < k1 ? (k1 - k0 + TC_TILE - 1) / TC_TILE : 0;
+    // the partial row of column gi: (b, query head, token)
+    auto prow = [&](int gi) -> size_t {
+      if constexpr (MULTI) {
+        const int c = g0 + gi;
+        return ((size_t)b * p.heads + (size_t)(c / p.tokens) * p.kv_heads + kvh) * p.tokens + c % p.tokens;
+      } else {
+        return (size_t)b * p.heads + (size_t)(g0 + gi) * p.kv_heads + kvh;
+      }
+    };
+    auto orow = [&](int gi) -> size_t {  // the same row, as the single-token epilogue has always computed it
+      if constexpr (MULTI) {
+        return prow(gi);
+      } else {
+        const int head = (g0 + gi) * p.kv_heads + kvh;
+        return (size_t)b * p.heads + head;
+      }
+    };
+    // multi-token: tiles inside [lo_in, hi_in) are visible to every token of the call and skip the per-column masks
+    int lo_in = 0, hi_in = 0;
+    if constexpr (MULTI) {
+      lo_in = td_col_range(p, b, p.tokens - 1, lo, k1).lo;
+      hi_in = td_col_range(p, b, 0, lo, k1).hi;
+      if (tid < NH) {
+        const TdColRange cr = td_col_range(p, b, (g0 + tid) % p.tokens, lo, k1);
+        sm.clo[tid] = tid < g ? cr.lo : 0;
+        sm.chi[tid] = tid < g ? cr.hi : 0;
+      }
+    }
     const float* ksb = p.k_scale ? p.k_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
     const float* vsb = p.v_scale ? p.v_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
 
@@ -168,7 +207,7 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
       const int gi = i / (D / 2), c = 2 * (i % (D / 2));
       float a = 0.f, bq = 0.f;
       if (gi < g) {
-        const size_t qi = ((size_t)b * p.heads + (size_t)(g0 + gi) * p.kv_heads + kvh) * D + c;
+        const size_t qi = prow(gi) * D + c;
         a = load_q(p.q, p.q_kind, qi);
         bq = load_q(p.q, p.q_kind, qi + 1);
       }
@@ -235,10 +274,16 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
       float cmax[2 * NJ];
 #pragma unroll
       for (int c = 0; c < 2 * NJ; ++c) cmax[c] = -INFINITY;
+      const bool edge = MULTI && (t0 < lo_in || t0 + TC_TILE > hi_in);
 #pragma unroll
       for (int i = 0; i < NH / 2; ++i) {
         const int key = t0 + r_lo + 8 * ((i >> 1) & 1);
-        if constexpr (RANGED) {
+        if constexpr (MULTI) {
+          float x = s[i] * ks;
+          if (p.softclamp_log2 > 0.f) x = fast_tanh(x * clamp_inv) * p.softclamp_log2;
+          const int col = 8 * (i / 4) + cq + (i & 1);
+          s[i] = !edge || (key >= sm.clo[col] && key < sm.chi[col]) ? x : -INFINITY;
+        } else if constexpr (RANGED) {
           float x = s[i] * ks;
           if (p.softclamp_log2 > 0.f) x = fast_tanh(x * clamp_inv) * p.softclamp_log2;
           s[i] = (key >= lo && key < k1) ? x : -INFINITY;  // a select: a NaN logit of a masked key goes too
@@ -335,13 +380,11 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
       for (int i = tid; i < g * D; i += TC_THREADS) {
         const int gi = i / D, c = i % D;
         const float l = sm.ml[1][gi];
-        const int head = (g0 + gi) * p.kv_heads + kvh;
-        my_partial[((size_t)b * p.heads + head) * row_stride + c] = l > 0.f ? sm.o[gi][c] / l : 0.f;
+        my_partial[orow(gi) * row_stride + c] = l > 0.f ? sm.o[gi][c] / l : 0.f;
       }
       if (tid < g) {
         const float l = sm.ml[1][tid], m = sm.ml[0][tid];
-        const int head = (g0 + tid) * p.kv_heads + kvh;
-        float* row = my_partial + ((size_t)b * p.heads + head) * row_stride;
+        float* row = my_partial + orow(tid) * row_stride;
         row[D] = l > 0.f ? (m == -INFINITY ? 0.f : m) + log2f(l) : -INFINITY;
         row[D + 1] = l > 0.f ? 1.f : 0.f;
       }
@@ -374,8 +417,7 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
             const float ms = __ldcg(&base[s * stride + D]);
             l += ms == -INFINITY ? 0.f : __ldcg(&base[s * stride + D + 1]) * fast_exp2(ms - m_eff);
           }
-          const int head = (g0 + gi) * p.kv_heads + kvh;
-          float* row = my_partial + ((size_t)b * p.heads + head) * row_stride;
+          float* row = my_partial + orow(gi) * row_stride;
           for (int c = tid; c < D; c += TC_THREADS) {
             float a = 0.f;
             for (int s = 0; s < p.splits; ++s) {
@@ -393,13 +435,31 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
     }
     __syncthreads();
   }
-  td_cross_rank_merge<D>(p, cs, total_units);
+  td_cross_rank_merge<D, MULTI>(p, cs, total_units);
 }
 
 template <int KVK, bool RANGED>
 const void* tc_ptr_nh(bool small_group) {
   return small_group ? (const void*)tree_decode_tc_kernel<KVK, 8, RANGED>
                      : (const void*)tree_decode_tc_kernel<KVK, 16, RANGED>;
+}
+// multi-token calls: NH = 8, 16 or 32 columns per unit for g * tokens <= 8, <= 16, larger
+int tc_multi_nh(int cols) { return cols <= 8 ? 8 : (cols <= 16 ? 16 : 32); }
+template <int KVK>
+const void* tc_ptr_multi(int nh) {
+  if (nh == 8) return (const void*)tree_decode_tc_kernel<KVK, 8, true, true>;
+  if (nh == 16) return (const void*)tree_decode_tc_kernel<KVK, 16, true, true>;
+  return (const void*)tree_decode_tc_kernel<KVK, 32, true, true>;
+}
+const void* pick_tc_multi(int kv_kind, int nh) {
+  if (kv_kind == 2) return tc_ptr_multi<2>(nh);
+  return kv_kind == 1 ? tc_ptr_multi<1>(nh) : tc_ptr_multi<0>(nh);
+}
+template <bool KV8>
+size_t tc_smem_multi(int nh) {
+  if (nh == 8) return sizeof(TcSmemMulti<KV8, 8>) + 1024;
+  if (nh == 16) return sizeof(TcSmemMulti<KV8, 16>) + 1024;
+  return sizeof(TcSmemMulti<KV8, 32>) + 1024;
 }
 template <bool RANGED>
 const void* pick_tc_r(int kv_kind, bool small_group) {
@@ -418,10 +478,13 @@ size_t tc_smem(int kv_kind, bool small_group) {
 
 }  // namespace
 
-int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged) {
+int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged, int cols) {
   const bool small = false;  // the 16-head variant: the larger shared-memory footprint bounds residency
-  const void* fn = pick_tc(kv_kind, small, ranged);
-  const size_t smem = tc_smem(kv_kind, small);
+  // a multi-token call plans with the residency of the variant it launches
+  const int nh = tc_multi_nh(cols);
+  const void* fn = cols > 0 ? pick_tc_multi(kv_kind, nh) : pick_tc(kv_kind, small, ranged);
+  const size_t smem = cols > 0 ? (kv_kind == 2 ? tc_smem_multi<true>(nh) : tc_smem_multi<false>(nh))
+                               : tc_smem(kv_kind, small);
   cuda_check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tree_decode_tc smem attr");
   int per_sm = 0;
   cuda_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, TC_THREADS, smem), "tree_decode_tc occupancy");
@@ -431,8 +494,11 @@ int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged) {
 void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, const TreeDecodeParams& p, int grid,
                            cudaStream_t stream, bool ranged) {
   const bool small = p.heads / p.kv_heads <= 8;
-  const void* fn = pick_tc(p.kv_kind, small, ranged);
-  const size_t smem = tc_smem(p.kv_kind, small);
+  const bool multi = p.tokens > 1;
+  const int nh = tc_multi_nh(p.heads / p.kv_heads * p.tokens);
+  const void* fn = multi ? pick_tc_multi(p.kv_kind, nh) : pick_tc(p.kv_kind, small, ranged);
+  const size_t smem = multi ? (p.kv_kind == 2 ? tc_smem_multi<true>(nh) : tc_smem_multi<false>(nh))
+                            : tc_smem(p.kv_kind, small);
   cuda_check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tree_decode_tc smem attr");
   void* args[] = {(void*)&map_k, (void*)&map_v, (void*)&p};
   // cooperative: the grid barrier and the cross-rank waits need every CTA of the grid to be resident

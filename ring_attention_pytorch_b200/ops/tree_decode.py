@@ -1,7 +1,8 @@
 """Tree-attention decoding: single-query attention over a KV cache sharded along the sequence across ranks
 (reference tree_attn_decoding.py:23-104, Algorithm 3 of https://arxiv.org/abs/2408.04093).
 
-Layout is head-first like the reference: ``q [b, h, 1, d]``, ``k [b, hk, n, d]``, ``v [b, hk, n, dv]``.
+Layout is head-first like the reference: ``q [b, h, m, d]`` (``m`` query tokens per sequence, 1 for plain decode),
+``k [b, hk, n, d]``, ``v [b, hk, n, dv]``.
 
 * CUDA path: ``csrc/tree_decode_tc_sm90.cu`` (head dim 128) / ``csrc/tree_decode_sm90.cu`` – ONE persistent cooperative kernel per rank and step computes the
   split-KV partials of its KV shard, merges the splits, publishes ``(out, lse)`` in symmetric memory, signals the
@@ -22,18 +23,19 @@ import torch.distributed as dist
 from torch import Tensor
 
 from ring_attention_pytorch_b200.parallel.distributed import default, exists, get_rank, get_world_size, is_distributed
-from ring_attention_pytorch_b200.utils.validate import check_decode_ranges, check_sinks, typecheck
+from ring_attention_pytorch_b200.utils.validate import check_decode_query, check_decode_ranges, check_sinks, typecheck
 
 
 def _visible_keys(n: int, cache_seqlens: Optional[Tensor], q_pos: Optional[Tensor], window: Optional[int],
-                  kv_pos: tuple[int, int], b: int, device) -> Tensor:
-    """bool [b, n]: local key j of sequence b is visible (see :func:`tree_attn_decode`)."""
+                  kv_pos: tuple[int, int], b: int, device, m: int = 1) -> Tensor:
+    """bool [b, m, n]: local key j of sequence b is visible to its query token t (see :func:`tree_attn_decode`)."""
     j = torch.arange(n, device=device, dtype=torch.int64)
-    vis = torch.ones(b, n, dtype=torch.bool, device=device)
+    vis = torch.ones(b, m, n, dtype=torch.bool, device=device)
     if cache_seqlens is not None:
-        vis &= j[None] < cache_seqlens.to(torch.int64)[:, None]
+        vis &= j[None, None] < cache_seqlens.to(torch.int64)[:, None, None]
     if q_pos is not None:
-        rel = q_pos.to(torch.int64)[:, None] - (kv_pos[0] + kv_pos[1] * j)[None]
+        t = torch.arange(m, device=device, dtype=torch.int64)
+        rel = (q_pos.to(torch.int64)[:, None] + t[None])[:, :, None] - (kv_pos[0] + kv_pos[1] * j)[None, None]
         vis &= rel >= 0
         if window is not None and window > 0:
             vis &= rel <= window
@@ -41,28 +43,29 @@ def _visible_keys(n: int, cache_seqlens: Optional[Tensor], q_pos: Optional[Tenso
 
 
 def _local_attention(q: Tensor, k: Tensor, v: Tensor, visible: Optional[Tensor] = None, softclamp_value: float = 0.0):
-    """q [b,h,1,d], k [b,hk,n,d], v [b,hk,n,dv] -> (out [b,h,1,dv] fp32, lse [b,h,1,1] fp32).  ``visible`` (bool
-    [b, n]) masks keys; a row that sees none gives out 0 and the finite sentinel lse ``-finfo.max``, so that the
-    cross-rank merge of a row empty on every rank computes exp(0), never -inf - -inf."""
-    b, h, _, d = q.shape
+    """q [b,h,m,d], k [b,hk,n,d], v [b,hk,n,dv] -> (out [b,h,m,dv] fp32, lse [b,h,m,1] fp32).  ``visible`` (bool
+    [b, m, n]) masks keys per query token; a row that sees none gives out 0 and the finite sentinel lse
+    ``-finfo.max``, so that the cross-rank merge of a row empty on every rank computes exp(0), never -inf - -inf."""
+    b, h, m, d = q.shape
     hk = k.shape[1]
     g = h // hk
     scale = d ** -0.5
-    qf = q.float().view(b, g, hk, 1, d)  # query head j uses kv head j % hk
+    qf = q.float().view(b, g, hk, m, d)  # query head j uses kv head j % hk
     sim = torch.einsum("bghid,bhjd->bghij", qf, k.float()) * scale
     if visible is not None:
         if softclamp_value > 0:
             sim = (sim / softclamp_value).tanh() * softclamp_value
-        sim = sim.masked_fill(~visible[:, None, None, None, :], -float("inf"))
+        sim = sim.masked_fill(~visible[:, None, None, :, :], -float("inf"))
         lse = sim.logsumexp(dim=-1, keepdim=True)
         lse = torch.where(lse == -float("inf"), torch.full_like(lse, -torch.finfo(torch.float32).max), lse)
-        vf = v.float().masked_fill(~visible[:, None, :, None], 0.0)  # 0 * NaN is NaN: invisible rows may hold anything
+        # 0 * NaN is NaN: keys no token sees may hold anything
+        vf = v.float().masked_fill(~visible.any(1)[:, None, :, None], 0.0)
         out = torch.einsum("bghij,bhjd->bghid", (sim - lse).exp(), vf)
-        return out.reshape(b, h, 1, -1), lse.reshape(b, h, 1, 1)
+        return out.reshape(b, h, m, -1), lse.reshape(b, h, m, 1)
     lse = sim.logsumexp(dim=-1, keepdim=True)
     attn = (sim - lse).exp()
     out = torch.einsum("bghij,bhjd->bghid", attn, v.float())
-    return out.reshape(b, h, 1, -1), lse.reshape(b, h, 1, 1)
+    return out.reshape(b, h, m, -1), lse.reshape(b, h, m, 1)
 
 
 @torch.no_grad()
@@ -82,7 +85,7 @@ def tree_attn_decode(
     softclamp_value: float = 0.0,
     kv_pos: Optional[tuple[int, int]] = None,
 ) -> Tensor:
-    """Returns ``[b, h, 1, dv]`` in ``q.dtype``.
+    """``q [b, h, m, d]``; returns ``[b, h, m, dv]`` in ``q.dtype``.
 
     ``shard_kv_seq=True``: every rank passes the *full* K/V and attends to its own ``chunk(world)`` slice
     (ranks beyond the number of chunks contribute nothing).  ``shard_kv_seq=False``: K/V are already this
@@ -100,10 +103,17 @@ def tree_attn_decode(
     ``kv_pos = (offset, stride)`` places its keys (required with ``q_pos`` on more than one rank; e.g. ``(rank,
     world)`` for round-robin appends).  ``softclamp_value > 0``: logits ``c * tanh(s / c)`` (the sink is not clamped).
     A row that sees no key on any rank and has no sink gives 0.
+
+    Multi-token decode (``m > 1``, e.g. verifying ``m`` draft tokens in one pass over the cache): query token ``t``
+    sits at ``q_pos[b] + t`` and sees key ``j`` iff the rule above holds at that position, so the tokens are causal
+    among themselves.  The caller appends the tokens' K/V first and counts them in ``cache_seqlens``.  Without
+    ``q_pos`` there is no position rule and every token sees every held key -- speculative verification needs
+    ``q_pos``.  GQA, softclamp, sinks (once per token row) and the cache formats apply per token row.
     """
     assert not (exists(k) ^ exists(v)), "keys and values are either both None, or both present"
+    check_decode_query(q, name="tree_attn_decode")
     dtype = q.dtype
-    b, h = q.shape[:2]
+    b, h, m = q.shape[:3]
     check_sinks(sinks, h, q.device, name="tree_attn_decode")
     check_decode_ranges(b, q.device, cache_seqlens, q_pos, window, kv_pos, softclamp_value, name="tree_attn_decode")
     ranged = exists(cache_seqlens) or exists(q_pos) or softclamp_value > 0
@@ -140,13 +150,13 @@ def tree_attn_decode(
         return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps, sinks=sinks).to(dtype)
 
     if exists(k) and k.shape[-2] > 0 and ranged:
-        visible = _visible_keys(k.shape[-2], cache_seqlens, q_pos, window, kv_pos, b, q.device)
+        visible = _visible_keys(k.shape[-2], cache_seqlens, q_pos, window, kv_pos, b, q.device, m)
         local_out, lse = _local_attention(q, k, v, visible, softclamp_value)
     elif exists(k) and k.shape[-2] > 0:
         local_out, lse = _local_attention(q, k, v)
     else:
-        local_out = q.new_zeros((b, h, 1, dim_v), dtype=torch.float32)
-        lse = torch.full((b, h, 1, 1), -torch.finfo(torch.float32).max, device=q.device, dtype=torch.float32)
+        local_out = q.new_zeros((b, h, m, dim_v), dtype=torch.float32)
+        lse = torch.full((b, h, m, 1), -torch.finfo(torch.float32).max, device=q.device, dtype=torch.float32)
 
     if not is_distributed() and not exists(sinks):
         return local_out.to(dtype)

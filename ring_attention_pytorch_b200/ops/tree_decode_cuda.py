@@ -19,7 +19,7 @@ from torch import Tensor
 
 from ring_attention_pytorch_b200.ops import _ext
 from ring_attention_pytorch_b200.parallel.distributed import get_rank, get_world_size, is_distributed
-from ring_attention_pytorch_b200.utils.validate import check_decode_ranges
+from ring_attention_pytorch_b200.utils.validate import check_decode_query, check_decode_ranges
 
 LAUNCHES = {"count": 0}
 # nvls "auto": use the NVSwitch multicast mapping when torch's symmetric memory can provide one, else NVLink peer loads
@@ -47,23 +47,32 @@ class DecodePlan:
     splits: int        # key splits per group
 
 
-def decode_span(n: int, window: Optional[int] = None, kv_pos_stride: int = 1) -> int:
+def decode_span(n: int, window: Optional[int] = None, kv_pos_stride: int = 1, tokens: int = 1) -> int:
     """The most keys, with the up-to-63-key slack of tile alignment, that one sequence's visible range can touch: the
     ranged kernels split this span, not ``n``.  With a look-back window a query sees at most ``window // stride + 1``
-    local keys, so the splits cover O(window) keys."""
+    local keys, so the splits cover O(window) keys; ``tokens`` consecutive queries see the union of their ranges, at
+    most ``(window + tokens - 1) // stride + 1`` keys."""
     if window is None or window <= 0:
         return n
-    return min(n, window // kv_pos_stride + TILE)
+    return min(n, (window + tokens - 1) // kv_pos_stride + TILE)
 
 
 def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int, *, ranged: bool = False,
-                span: Optional[int] = None) -> DecodePlan:
+                span: Optional[int] = None, tokens: int = 1) -> DecodePlan:
     """The kernel and the work split a decode call of these sizes gets (``kv_kind``: 0 bf16, 1 fp16, 2 fp8 cache).
     ``ranged``: the instantiations with per-sequence key ranges / softclamp; ``span`` (default ``n``): the keys the
-    splits are planned over (:func:`decode_span`)."""
+    splits are planned over (:func:`decode_span`).  ``tokens > 1``: a multi-token call (always ranged), whose work
+    units hold ``NH`` (query head, token) columns of one kv head -- 8, 16 or 32 for ``g * tokens`` up to 8, up to 16,
+    larger on the tensor-core kernel, 4 on the CUDA-core kernel -- planned with that variant's residency."""
     tc = CONFIG["tensor_core"]
     use_tc = tc in ("auto", True, "on") and d == 128 and n >= 1
     g = h // hk
+    if tokens > 1:
+        cols = g * tokens
+        gm = (8 if cols <= 8 else (16 if cols <= 16 else 32)) if use_tc else 4
+        groups = b * hk * ((cols + gm - 1) // gm)
+        resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc, True, cols))
+        return DecodePlan(use_tc, groups, resident, _choose_splits(n if span is None else span, groups, resident))
     gm = (8 if g <= 8 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: MMA N)
     groups = b * hk * ((g + gm - 1) // gm)
     resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc))
@@ -157,8 +166,8 @@ def _buffers(rows: int, d: int, dev: torch.device) -> _Buffers:
 
 def uses_nvls(q: Tensor) -> bool:
     """True when the decode of this (shape, device) merges through the NVSwitch multicast mapping."""
-    b, h, _, d = q.shape
-    key = (q.device.index, get_world_size() if is_distributed() else 1, b * h, d)
+    b, h, m, d = q.shape
+    key = (q.device.index, get_world_size() if is_distributed() else 1, b * h * m, d)
     return key in _cache and _cache[key].mc_partial_ptr != 0
 
 
@@ -192,15 +201,16 @@ def tree_decode_cuda(
     kv_pos: Tuple[int, int] = (0, 1),
     softclamp_value: float = 0.0,
 ) -> Tensor:
-    """q [b, h, 1, d] (bf16 / fp16 / fp32); k, v [b, hk, n, d] this rank's shard (bf16 / fp16 / float8_e4m3fn) or None.
+    """q [b, h, m, d] (bf16 / fp16 / fp32; m >= 1 query tokens per sequence); k, v [b, hk, n, d] this rank's shard
+    (bf16 / fp16 / float8_e4m3fn) or None.
     k / v may be the filled prefix ``cache[:, :, :n]`` of a larger ``[b, hk, capacity, d]`` buffer: the tensor-core kernel
     (head dim 128, n >= 128) reads it in place; other cases are made contiguous first.
 
     ``k_scale`` / ``v_scale``: optional fp32 dequantisation scales for the fp8 path, either per (batch, kv head)
     (``numel == b*hk``) or block-scaled ``[b*hk, n_blocks]`` with one scale per ``scale_block_keys`` keys
-    (a multiple of 64).  ``out`` ([b, h, 1, d]) may be passed to make the call allocation free (CUDA graphs).
-    ``sinks`` (``[h]``, fp32 contiguous for an allocation-free call): learned attention sinks, added once, in the
-    kernel's cross-rank merge.  Returns [b, h, 1, d] in q's dtype.
+    (a multiple of 64).  ``out`` ([b, h, m, d]) may be passed to make the call allocation free (CUDA graphs).
+    ``sinks`` (``[h]``, fp32 contiguous for an allocation-free call): learned attention sinks, added once per token row,
+    in the kernel's cross-rank merge.  Returns [b, h, m, d] in q's dtype.
 
     Ragged and windowed decode.  Local key ``j`` sits at global position ``P(j) = kv_pos[0] + kv_pos[1] * j`` and is
     visible iff ``j < min(cache_seqlens[b], n)`` (int32 ``[b]``; None: every key), ``P(j) <= q_pos[b]`` (integer
@@ -208,14 +218,20 @@ def tree_decode_cuda(
     kernel derives each sequence's key range from the device tensors, so a decode loop can update them in place and
     replay a captured graph; the whole ``[b, hk, capacity, d]`` buffers may be passed.  ``softclamp_value > 0`` turns
     the logits into ``c * tanh(s / c)`` (not the sink).  A row that sees no key and has no sink gives 0.
+
+    Multi-token decode (``m > 1``, e.g. verifying ``m`` draft tokens): query token ``t`` sits at ``q_pos[b] + t`` and
+    each token applies the rule above at its own position, so the tokens are causal among themselves; their K / V are
+    appended (and counted in ``cache_seqlens``) before the call.  Without ``q_pos`` there is no position rule: every
+    token sees every held key.  One pass over the cache serves all ``m`` tokens.  ``q_pos + m - 1`` must fit in int32.
     """
+    check_decode_query(q, out, dim_v, name="tree_decode_cuda")
     ops = _ext.ops()
-    b, h, _, d = q.shape
+    b, h, m, d = q.shape
     check_decode_ranges(b, q.device, cache_seqlens, q_pos, window, kv_pos, softclamp_value, name="tree_decode_cuda")
-    ranged = cache_seqlens is not None or q_pos is not None or softclamp_value > 0
+    ranged = cache_seqlens is not None or q_pos is not None or softclamp_value > 0 or m > 1
     assert dim_v == d, "the decode kernel assumes dim_v == dim_qk"
     dev = q.device
-    q3 = q.reshape(b, h, d)
+    q3 = q.reshape(b, h, d) if m == 1 else q
     if not q3.is_contiguous():
         q3 = q3.contiguous()
     if q3.dtype not in (torch.bfloat16, torch.float16, torch.float32):
@@ -229,38 +245,42 @@ def tree_decode_cuda(
         k = v = None
     g = h // hk
     kv_kind = 0 if k is None or k.dtype == torch.bfloat16 else (1 if k.dtype == torch.float16 else 2)
-    if ranged:
+    if m > 1:
+        plan = decode_plan(b, h, hk, n, d, kv_kind, ranged=True, span=decode_span(n, window, int(kv_pos[1]), m),
+                           tokens=m)
+    elif ranged:
         plan = decode_plan(b, h, hk, n, d, kv_kind, ranged=True, span=decode_span(n, window, int(kv_pos[1])))
     else:
         plan = decode_plan(b, h, hk, n, d, kv_kind)
     use_tc, groups, resident, splits = plan.tensor_core, plan.groups, plan.resident, plan.splits
     if k is not None and not (use_tc and _is_cache_prefix(k) and v.stride() == k.stride()):
         k, v = k.contiguous(), v.contiguous()  # no-op for dense inputs
-    buf = _buffers(b * h, d, dev)
-    need = b * hk * splits * g * (d + 4)
+    buf = _buffers(b * h * m, d, dev)
+    need = b * hk * splits * g * m * (d + 4)  # scratch rows: (b, kv head, split, column), g * m columns
     if buf.scratch is None or buf.scratch.numel() < need:
         buf.scratch = torch.empty(need, dtype=torch.float32, device=dev)
-    if buf.group_done is None or buf.group_done.numel() < b * hk * ((g + 3) // 4):
-        buf.group_done = torch.zeros(b * hk * ((g + 3) // 4), dtype=torch.int32, device=dev)
+    if buf.group_done is None or buf.group_done.numel() < b * hk * ((g * m + 3) // 4):
+        buf.group_done = torch.zeros(b * hk * ((g * m + 3) // 4), dtype=torch.int32, device=dev)
     if out is None:
         out_dtype = q.dtype if q.dtype in (torch.bfloat16, torch.float16) else torch.float32
-        out = torch.empty(b, h, 1, d, dtype=out_dtype, device=dev)
+        out = torch.empty(b, h, m, d, dtype=out_dtype, device=dev)
     if sinks is not None:
         sinks = sinks.float().contiguous()
     units = groups * splits if n > 0 else 0
-    grid = max(1, min(resident, max(units, (b * h + 3) // 4)))
+    grid = max(1, min(resident, max(units, (b * h * m + 3) // 4)))
+    out_k = out.view(b, h, d) if m == 1 else out
     if ranged:
         if q_pos is not None and q_pos.dtype != torch.int32:
             q_pos = q_pos.to(torch.int32)
         ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
-                        buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out.view(b, h, d),
+                        buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out_k,
                         hk, splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks,
                         cache_seqlens.contiguous() if cache_seqlens is not None else None, q_pos.contiguous()
                         if q_pos is not None else None, window or 0, int(kv_pos[0]), int(kv_pos[1]),
                         float(softclamp_value))
     else:
         ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
-                        buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out.view(b, h, d),
+                        buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out_k,
                         hk, splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks)
     LAUNCHES["count"] += 1
     return out

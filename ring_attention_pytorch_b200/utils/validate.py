@@ -71,6 +71,21 @@ def check_sinks(sinks: Optional[Tensor], heads: int, device, *, name: str = "att
         raise ValueError(f"{name}: sinks must live on {device}, got {sinks.device}")
 
 
+def check_decode_query(q, out=None, dim_v: Optional[int] = None, *, name: str = "decode") -> None:
+    """The query of a decode call: a 4-D ``[b, h, m, d]`` tensor with ``m >= 1`` query tokens per sequence, and
+    ``out`` (when given) ``[b, h, m, dim_v]``."""
+    if not torch.is_tensor(q) or q.dim() != 4:
+        raise ValueError(f"{name}: q must be a 4-D tensor [batch, heads, tokens, dim], got "
+                         f"{tuple(q.shape) if torch.is_tensor(q) else type(q)}")
+    if q.shape[2] < 1:
+        raise ValueError(f"{name}: q needs at least one query token per sequence, got shape {tuple(q.shape)}")
+    if out is not None:
+        want = (*q.shape[:3], q.shape[3] if dim_v is None else dim_v)
+        if not torch.is_tensor(out) or tuple(out.shape) != want:
+            raise ValueError(f"{name}: out must be {list(want)}, got "
+                             f"{tuple(out.shape) if torch.is_tensor(out) else type(out)}")
+
+
 def check_decode_ranges(batch: int, device, cache_seqlens: Optional[Tensor], q_pos: Optional[Tensor],
                         window: Optional[int], kv_pos, softclamp_value: float, *, name: str = "decode") -> None:
     """Per-sequence key ranges of a decode call: ``cache_seqlens`` int32 ``[batch]``, ``q_pos`` integer ``[batch]``,
