@@ -20,6 +20,9 @@ tokens are appended round-robin so that the shards stay balanced.
 
     # speculative verification: every step appends 4 draft tokens and checks them in one decode call
     ... examples/decode_tree_attention.py --context 1048576 --batch 16 --draft 4
+
+    # paged KV cache: 16-token pages from a shuffled free list, pages behind the window go back to the list
+    ... examples/decode_tree_attention.py --context 1048576 --batch 16 --ragged --window 4096 --page-size 16
 """
 from __future__ import annotations
 
@@ -50,6 +53,8 @@ def parse_args(argv=None):
     ap.add_argument("--window", type=int, default=None, help="look-back window: the query sees positions >= pos - W")
     ap.add_argument("--draft", type=int, default=1,
                     help="query tokens per step: append M tokens and decode them in one call (causal among themselves)")
+    ap.add_argument("--page-size", type=int, default=None,
+                    help="paged KV cache: each rank keeps a pool of pages of P tokens and a block table per sequence")
     return ap.parse_args(argv)
 
 
@@ -73,7 +78,7 @@ class ShardedKVCache:
 
 def run(args) -> float:
     """Inside an initialised process group.  Returns the largest error seen with ``--check`` (0.0 otherwise)."""
-    if args.ragged or args.window is not None or args.draft > 1:
+    if args.ragged or args.window is not None or args.draft > 1 or args.page_size:
         return run_ragged(args)
     from ring_attention_pytorch_b200 import tree_attn_decode
 
@@ -162,7 +167,11 @@ def run_ragged(args) -> float:
     """``--ragged`` / ``--window`` / ``--draft``: every sequence has its own length, the decode passes the whole capacity
     buffers with per-sequence ``cache_seqlens``, query positions and ``kv_pos = (rank, world)`` (token t of a sequence
     lives on rank t % world at local slot t // world).  Slots past a sequence's length hold NaN (0x7F in e4m3): they
-    must not matter.  Each step appends ``--draft`` tokens and decodes all of them in one call."""
+    must not matter.  Each step appends ``--draft`` tokens and decodes all of them in one call.
+
+    ``--page-size P``: each rank keeps K / V in a pool of P-token pages and a block table per sequence.  Pages come from
+    a seeded, shuffled free list as a sequence grows; with a window, pages wholly behind every future query's window go
+    back to the list (and may be handed to another sequence) while the table still names them."""
     from ring_attention_pytorch_b200 import tree_attn_decode
     from ring_attention_pytorch_b200.ops.oracle import attention_with_positions
     from ring_attention_pytorch_b200.ops.tree_decode_cuda import tree_decode_cuda
@@ -195,14 +204,37 @@ def run_ragged(args) -> float:
         dist.all_reduce(k_scale, dist.ReduceOp.MAX)
         dist.all_reduce(v_scale, dist.ReduceOp.MAX)
         pk, pv = pk / k_scale.view(b, hk, 1, 1), pv / v_scale.view(b, hk, 1, 1)
-    kc = torch.empty(b, hk, cap, d, dtype=cache_dtype, device=dev)
+    held = local_len(lens)
+    P = args.page_size
+    if P:
+        from ring_attention_pytorch_b200 import write_paged_kv
+
+        max_pages = (cap + P - 1) // P
+        # a pool with room for every sequence's pages; ids handed out in a seeded random order
+        kc = torch.empty(b * max_pages + 1, hk, P, d, dtype=cache_dtype, device=dev)
+        free = torch.randperm(kc.shape[0], generator=torch.Generator().manual_seed(args.seed + 101 + rank)).tolist()
+        table = torch.zeros(b, max_pages, dtype=torch.int32)
+        owned = [0] * b  # pages [0, owned[i]) of sequence i are in the table
+        released = [0] * b  # pages [0, released[i]) went back to the free list
+
+        def grow(i, n):  # sequence i holds n local keys: give it the pages they need
+            while owned[i] * P < n:
+                table[i, owned[i]] = free.pop()
+                owned[i] += 1
+    else:
+        kc = torch.empty(b, hk, cap, d, dtype=cache_dtype, device=dev)
     vc = torch.empty_like(kc)
     for t in (kc, vc):
         (t.view(torch.uint8).fill_(0x7F) if args.fp8 else t.fill_(float("nan")))
-    held = local_len(lens)
     for i in range(b):
-        kc[i, :, :held[i]] = pk[i, :, :held[i]].to(cache_dtype)
-        vc[i, :, :held[i]] = pv[i, :, :held[i]].to(cache_dtype)
+        if P:
+            grow(i, int(held[i]))
+            tb = table[i:i + 1].to(dev)
+            write_paged_kv(kc, vc, tb, torch.zeros(1, dtype=torch.int64, device=dev), pk[i:i + 1, :, :held[i]],
+                           pv[i:i + 1, :, :held[i]])
+        else:
+            kc[i, :, :held[i]] = pk[i, :, :held[i]].to(cache_dtype)
+            vc[i, :, :held[i]] = pv[i, :, :held[i]].to(cache_dtype)
     del pk, pv
 
     def quantised(t, scale):  # what the cache stores, as fp32 (for --check)
@@ -214,7 +246,13 @@ def run_ragged(args) -> float:
         total = int(lens.max()) + args.steps * M
         full_k, full_v = torch.zeros(b, hk, total, d), torch.zeros(b, hk, total, d)
         parts = [None] * world
-        dist.all_gather_object(parts, (quantised(kc.float(), k_scale).cpu(), quantised(vc.float(), v_scale).cpu()))
+        if P:
+            from ring_attention_pytorch_b200 import gather_paged_kv
+
+            kg, vg = gather_paged_kv(kc, table.to(dev)), gather_paged_kv(vc, table.to(dev))
+        else:
+            kg, vg = kc, vc
+        dist.all_gather_object(parts, (quantised(kg.float(), k_scale).cpu(), quantised(vg.float(), v_scale).cpu()))
         for r, (pk_r, pv_r) in enumerate(parts):
             for i in range(b):
                 m = len(range(r, int(lens[i]), world))
@@ -230,6 +268,12 @@ def run_ragged(args) -> float:
             pos = lens + u
             mine = (pos % world == rank).nonzero().flatten()
             slot = local_len(pos)[mine]
+            if P:
+                for i, s_ in zip(mine.tolist(), slot.tolist()):
+                    grow(i, s_ + 1)
+                write_paged_kv(kc, vc, table[mine].to(dev), slot.to(dev), k_new[mine, :, u:u + 1].to(dev),
+                               v_new[mine, :, u:u + 1].to(dev))
+                continue
             kc[mine.to(dev), :, slot.to(dev)] = k_new[mine, :, u].to(dev, cache_dtype)
             vc[mine.to(dev), :, slot.to(dev)] = v_new[mine, :, u].to(dev, cache_dtype)
         q_pos = lens.clone()  # the first new token's position
@@ -237,6 +281,8 @@ def run_ragged(args) -> float:
         held = local_len(lens)
         kw = dict(cache_seqlens=held.to(dev, torch.int32), q_pos=q_pos.to(dev, torch.int32), window=args.window,
                   kv_pos=(rank, world))
+        if P:
+            kw["block_table"] = table.to(dev)
         seen += int(sum(min(int(n), (args.window or int(n)) + M) for n in lens))
         if cuda:
             torch.cuda.synchronize(dev)
@@ -248,6 +294,14 @@ def run_ragged(args) -> float:
         if cuda:
             torch.cuda.synchronize(dev)
         times.append(time.perf_counter() - t0)
+        if P and args.window is not None:
+            # every later query sits at >= lens: local keys before the first one its window reaches are dead, and so
+            # is every page that holds only such keys (the table keeps naming it; the kernels never read it)
+            first = local_len((lens - args.window).clamp(min=0))
+            for i in range(b):
+                while (released[i] + 1) * P <= int(first[i]) and released[i] < owned[i]:
+                    free.append(int(table[i, released[i]]))  # handed out next, to any sequence
+                    released[i] += 1
         if args.check:
             kq = quantised(k_new, k_scale.cpu() if k_scale is not None else None)
             vq = quantised(v_new, v_scale.cpu() if v_scale is not None else None)

@@ -13,6 +13,7 @@ from ring_attention_pytorch_b200.models.ring_attention import (
 )
 from ring_attention_pytorch_b200.ops.flash_attn import flash_attn_backward, flash_attn_forward
 from ring_attention_pytorch_b200.ops.oracle import attention_with_positions, default_attention
+from ring_attention_pytorch_b200.ops.paged_kv import gather_paged_kv, write_paged_kv
 from ring_attention_pytorch_b200.ops.ring_flash_naive import ring_flash_attn, ring_flash_attn_
 from ring_attention_pytorch_b200.ops.tree_decode import tree_attn_decode
 from ring_attention_pytorch_b200.ops.zig_zag import zig_zag_attn, zig_zag_pad_seq, zig_zag_shard
@@ -47,6 +48,8 @@ __all__ = [
     "ring_flash_attn_fp8",
     "quantize_fp8",
     "tree_attn_decode",
+    "gather_paged_kv",
+    "write_paged_kv",
     "flash_attn_forward",
     "flash_attn_backward",
     "zig_zag_attn",

@@ -570,9 +570,10 @@ void acc_convert(const Tensor& acc, Tensor out, double scale) {
 // (ops/tree_decode_cuda.py caches them), so the call allocates nothing and can be captured in a CUDA graph.
 // ---------------------------------------------------------------------------------------------
 // cols > 0: a multi-token call with g * tokens (query head, token) columns per kv head
-int64_t tree_decode_max_ctas(int64_t d, int64_t kv_kind, bool tensor_core, bool ranged, int64_t cols) {
-  if (tensor_core) return rab::tree_decode_tc_max_ctas((int)kv_kind, sm_count(), ranged, (int)cols);
-  return rab::tree_decode_max_ctas((int)d, (int)kv_kind, sm_count(), ranged, cols > 0);
+// paged: the residency of the paged instantiation a call with a block table launches
+int64_t tree_decode_max_ctas(int64_t d, int64_t kv_kind, bool tensor_core, bool ranged, int64_t cols, bool paged) {
+  if (tensor_core) return rab::tree_decode_tc_max_ctas((int)kv_kind, sm_count(), ranged, (int)cols, paged);
+  return rab::tree_decode_max_ctas((int)d, (int)kv_kind, sm_count(), ranged, cols > 0, paged);
 }
 
 // int32 [b] on q's device (ranged decode: per-sequence cache lengths / query positions), or null
@@ -591,7 +592,7 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
                  int64_t kv_heads, int64_t splits, double scale, int64_t scale_block_keys, double eps, int64_t grid,
                  bool tensor_core, const c10::optional<Tensor>& sinks, const c10::optional<Tensor>& cache_seqlens,
                  const c10::optional<Tensor>& q_pos, int64_t window, int64_t kv_pos_offset, int64_t kv_pos_stride,
-                 double softclamp) {
+                 double softclamp, const c10::optional<Tensor>& block_table) {
   TORCH_CHECK(q.is_cuda() && q.is_contiguous() && (q.dim() == 3 || q.dim() == 4),
               "q must be contiguous [b, h, d] or [b, h, tokens, d]");
   const int b = q.size(0), h = q.size(1), d = q.size(-1);
@@ -605,7 +606,40 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   TORCH_CHECK(p.q_kind != 2 || q.scalar_type() == at::kFloat, "q must be bf16, fp16 or fp32");
   int n = 0;
   int64_t kv_plane_stride = 0;  // elements between consecutive (batch, kv head) planes
-  if (k.has_value()) {
+  const bool paged = block_table.has_value();
+  TORCH_CHECK(!paged || k.has_value(), "block_table needs the k / v page pools");
+  if (paged) {
+    // page pools [num_pages, hk, page_size, d]: any page / head / slot strides (HND, or NHD seen as HND), unit d stride
+    TORCH_CHECK(v.has_value() && k->dim() == 4 && k->sizes() == v->sizes() && k->strides() == v->strides() &&
+                    k->scalar_type() == v->scalar_type(),
+                "k / v page pools must share shape, dtype and strides");
+    TORCH_CHECK(k->size(0) >= 1 && k->size(1) == kv_heads && k->size(3) == d && k->stride(3) == 1,
+                "page pools must be [num_pages, hk, page_size, d] with unit d stride");
+    const int64_t ps = k->size(2);
+    TORCH_CHECK(ps == 16 || ps == 32 || (ps > 0 && ps % 64 == 0), "page_size must be 16, 32 or a multiple of 64");
+    const Tensor& t = *block_table;
+    TORCH_CHECK(t.device() == q.device() && t.scalar_type() == at::kInt && t.dim() == 2 && t.size(0) == b &&
+                    t.size(1) >= 1 && t.is_contiguous(),
+                "block_table must be a contiguous int32 [batch, max_pages] tensor on q's device");
+    TORCH_CHECK(t.size(1) * ps < ((int64_t)1 << 31), "max_pages * page_size must be below 2^31");
+    const int64_t eb = k->element_size();
+    for (int i = 0; i < 3; ++i) TORCH_CHECK((k->stride(i) * eb) % 16 == 0, "pool strides must be multiples of 16 bytes");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(k->data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(v->data_ptr()) % 16 == 0,
+                "page pools must be 16-byte aligned");
+    n = (int)(t.size(1) * ps);
+    p.block_table = t.data_ptr<int>();
+    p.max_pages = (int)t.size(1);
+    p.page_size = (int)ps;
+    p.page_stride = k->stride(0);
+    p.head_stride = k->stride(1);
+    p.slot_stride = k->stride(2);
+    if (k->scalar_type() == at::kBFloat16) p.kv_kind = 0;
+    else if (k->scalar_type() == at::kHalf) p.kv_kind = 1;
+    else if (k->scalar_type() == at::kFloat8_e4m3fn) p.kv_kind = 2;
+    else TORCH_CHECK(false, "k/v must be bf16, fp16 or float8_e4m3fn");
+    p.k = k->data_ptr();
+    p.v = v->data_ptr();
+  } else if (k.has_value()) {
     TORCH_CHECK(v.has_value() && k->dim() == 4 && k->sizes() == v->sizes());
     TORCH_CHECK(k->is_contiguous() ? v->is_contiguous() : k->strides() == v->strides(), "k and v must share a layout");
     TORCH_CHECK(k->size(0) == b && k->size(1) == kv_heads && k->size(3) == d);
@@ -682,10 +716,25 @@ void tree_decode(const Tensor& q, const c10::optional<Tensor>& k, const c10::opt
   p.kv_pos_offset = (int)kv_pos_offset;
   p.kv_pos_stride = (int)kv_pos_stride;
   p.softclamp_log2 = (float)(softclamp * 1.4426950408889634);
-  // a multi-token call always takes the ranged body (its kernels derive per-token key ranges)
-  const bool ranged = p.cache_seqlens != nullptr || p.q_pos != nullptr || softclamp > 0.0 || tokens > 1;
+  TORCH_CHECK(!paged || p.cache_seqlens != nullptr, "a paged call needs cache_seqlens");
+  // a multi-token or paged call always takes the ranged body (its kernels derive per-token / per-sequence key ranges)
+  const bool ranged = p.cache_seqlens != nullptr || p.q_pos != nullptr || softclamp > 0.0 || tokens > 1 || paged;
   c10::cuda::CUDAGuard guard(q.device());
-  if (tensor_core) {
+  if (tensor_core && paged) {
+    TORCH_CHECK(d == 128, "the tensor-core decode kernel needs head dim 128");
+    // the pools as (d, page_size, hk, num_pages); box = one 128-byte wide sub-tile of min(page_size, 64) keys of a page
+    const uint64_t eb = p.kv_kind == 2 ? 1 : 2;
+    uint64_t dims[4] = {(uint64_t)d, (uint64_t)p.page_size, (uint64_t)kv_heads, (uint64_t)k->size(0)};
+    uint64_t strides[3] = {(uint64_t)p.slot_stride * eb, (uint64_t)p.head_stride * eb, (uint64_t)p.page_stride * eb};
+    uint32_t box[4] = {(uint32_t)(128 / eb), (uint32_t)std::min(p.page_size, 64), 1, 1};
+    auto mk = [&](const void* base) {
+      if (p.kv_kind == 2) return rab::make_tmap_u8(base, 4, dims, strides, box, rab::TmapSwizzle::B128);
+      if (p.kv_kind == 1) return rab::make_tmap_f16(base, 4, dims, strides, box, rab::TmapSwizzle::B128);
+      return rab::make_tmap_bf16(base, 4, dims, strides, box, rab::TmapSwizzle::B128);
+    };
+    CUtensorMap map_k = mk(p.k), map_v = mk(p.v);
+    rab::launch_tree_decode_tc(map_k, map_v, p, (int)grid, at::cuda::getCurrentCUDAStream(), ranged);
+  } else if (tensor_core) {
     TORCH_CHECK(d == 128 && n > 0, "the tensor-core decode kernel needs head dim 128 and a non-empty shard");
     // K, V [b*hk, n, d] with any plane stride (a growing cache is read in place) -> dims (d, n, b*hk);
     // box = one 128-byte wide, 64-key sub-tile
@@ -824,8 +873,9 @@ TORCH_LIBRARY(rab, m) {
         "group_done, Tensor(c!) counters, int[] partial_ptrs, int aux_local_ptr, int[] pad_ptrs, int mc_partial_ptr, int "
         "mc_aux_ptr, int rank, Tensor(d!) out, int kv_heads, int splits, float scale, int scale_block_keys, float eps, "
         "int grid, bool tensor_core, Tensor? sinks=None, Tensor? cache_seqlens=None, Tensor? q_pos=None, int window=0, "
-        "int kv_pos_offset=0, int kv_pos_stride=1, float softclamp=0.0) -> ()");
-  m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core, bool ranged=False, int cols=0) -> int");
+        "int kv_pos_offset=0, int kv_pos_stride=1, float softclamp=0.0, Tensor? block_table=None) -> ()");
+  m.def("tree_decode_max_ctas(int d, int kv_kind, bool tensor_core, bool ranged=False, int cols=0, bool paged=False) "
+        "-> int");
   m.def("bwd_prep(Tensor q, Tensor o, Tensor dout, Tensor lse, Tensor(a!) qdo_buf, Tensor(b!) stat_buf, int rank, "
         "Tensor? sinks=None, Tensor(c!)? dsinks=None) -> ()");
   m.def("attn_bwd_dq(Tensor qdo_buf, Tensor kv_buf, Tensor stat_buf, Tensor? ready, int ready_target, Tensor? "

@@ -209,13 +209,22 @@ struct TreeDecodeParams {
   // Token t sits at q_pos[b] + t (the position rule above per token); the work unit's columns are the g * tokens
   // (query head, token) pairs of one kv head, column c = (head slot c / tokens, token c % tokens).
   int tokens;
+  // Paged KV cache (the `paged` kernels, always ranged; null block_table: the fields are not read).  k / v are page pools
+  // [num_pages, hk, page_size, d] with element strides (page_stride, head_stride, slot_stride) and unit d stride; local
+  // key j of sequence b is slot j % page_size of page block_table[b * max_pages + j / page_size], n = max_pages *
+  // page_size.  Only entries of pages that hold a key of some unit's [lo, k1) are read.
+  const int* block_table;             // int32 [batch][max_pages], entries in [0, num_pages)
+  int max_pages, page_size;           // page_size: 16, 32 or a multiple of 64
+  long long page_stride, head_stride, slot_stride;
 };
-int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged, bool multi = false);
+// paged: plan with the residency of the paged instantiation (p.block_table != null launches it)
+int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged, bool multi = false, bool paged = false);
 // p.tokens > 1 launches the multi-token instantiations
 void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream, bool ranged);
-// wgmma variant (tree_decode_tc_sm90.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 64-key box.
+// wgmma variant (tree_decode_tc_sm90.cu): head dim 128; map_k / map_v: K, V as (d, n, b*hk) with a 128-byte x 64-key box,
+// or, paged, the pools as (d, page_size, hk, num_pages) with a 128-byte x min(page_size, 64)-key box.
 // cols: (query head, token) columns per kv head of a multi-token call (g * tokens), 0 for a single-token call
-int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged, int cols = 0);
+int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged, int cols = 0, bool paged = false);
 void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, const TreeDecodeParams& p, int grid,
                            cudaStream_t stream, bool ranged);
 

@@ -85,11 +85,13 @@ struct KvVec<2> {
 // RANGED: per-sequence visible key ranges and softclamp (TreeDecodeParams).  Key loads are clamped into [lo, k1), so a
 // masked key's probability of 0 always multiplies a visible (finite) value row.  MULTI (with RANGED): the 4 columns of a
 // unit are (query head, token) pairs of a multi-token call; the unit streams the union of its tokens' key ranges and
-// masks each column with its own token's range.
-template <int D, int KV_KIND, bool RANGED, bool MULTI = false>
-__global__ void __launch_bounds__(TD_THREADS)
-tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
+// masks each column with its own token's range.  PAGED (with RANGED): K / V rows come from page pools, each (clamped)
+// key's row addressed through block_table and the pool strides with 64-bit offsets; the clamp into [lo, k1) keeps every
+// table read on a page that holds a visible key.
+template <int D, int KV_KIND, bool RANGED, bool MULTI, bool PAGED>
+__device__ __forceinline__ void td_decode_body(const TreeDecodeParams& p) {
   static_assert(RANGED || !MULTI, "a multi-token call takes the ranged body");
+  static_assert(RANGED || !PAGED, "a paged call takes the ranged body");
   using Vec = KvVec<KV_KIND>;
   using Raw = typename Vec::Raw;
   const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
@@ -160,6 +162,15 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
     const float* vsb = p.v_scale ? p.v_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
     const uint8_t* kbase = reinterpret_cast<const uint8_t*>(p.k) + (size_t)bhk * p.n * D * eb;
     const uint8_t* vbase = reinterpret_cast<const uint8_t*>(p.v) + (size_t)bhk * p.n * D * eb;
+    // paged: the byte offset of key's row from kbase / vbase (the kv head's offset in the pools)
+    if constexpr (PAGED) {
+      kbase = reinterpret_cast<const uint8_t*>(p.k) + (size_t)kvh * p.head_stride * eb;
+      vbase = reinterpret_cast<const uint8_t*>(p.v) + (size_t)kvh * p.head_stride * eb;
+    }
+    auto page_off = [&](int key) -> size_t {
+      const int page = __ldg(p.block_table + (size_t)b * p.max_pages + key / p.page_size);
+      return ((size_t)page * p.page_stride + (size_t)(key % p.page_size) * p.slot_stride) * eb;
+    };
 
     float2 qr[TD_MAX_G][EPL / 2];  // packed pairs: two lanes of a pair per dot-product step
 #pragma unroll
@@ -187,7 +198,8 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
       for (int step = 0; step < 4; ++step) {
         int key = min(t0 + warp * 16 + step * 4 + sub, k1 - 1);  // clamp: loads stay in bounds
         if constexpr (RANGED) key = max(key, lo);
-        const uint8_t* row = kbase + ((size_t)key * D + l8 * EPL) * eb;
+        const uint8_t* row = PAGED ? kbase + page_off(key) + (size_t)l8 * EPL * eb
+                                   : kbase + ((size_t)key * D + l8 * EPL) * eb;
 #pragma unroll
         for (int c = 0; c < KVEC; ++c) kraw[step][c] = *reinterpret_cast<const Raw*>(row + c * Vec::kBytes);
       }
@@ -197,7 +209,8 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
       for (int i = 0; i < KPT; ++i) {
         int key = min(t0 + kgrp + i * KGROUPS, k1 - 1);
         if constexpr (RANGED) key = max(key, lo);
-        vraw[i] = *reinterpret_cast<const Raw*>(vbase + ((size_t)key * D + chunk * 8) * eb);
+        vraw[i] = *reinterpret_cast<const Raw*>(PAGED ? vbase + page_off(key) + (size_t)chunk * 8 * eb
+                                                       : vbase + ((size_t)key * D + chunk * 8) * eb);
       }
     };
     if (k0 < k1) {
@@ -396,6 +409,32 @@ tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
   td_cross_rank_merge<D, MULTI>(p, cs, total_units);
 }
 
+template <int D, int KV_KIND, bool RANGED, bool MULTI = false>
+__global__ void __launch_bounds__(TD_THREADS)
+tree_decode_kernel(const __grid_constant__ TreeDecodeParams p) {
+  td_decode_body<D, KV_KIND, RANGED, MULTI, false>(p);
+}
+
+// paged K / V (TreeDecodeParams::block_table): always the ranged body.  Two CTAs per SM: without the hint ptxas caps the
+// head-dim-64 fp8 variant at 128 registers and spills.
+template <int D, int KV_KIND, bool MULTI>
+__global__ void __launch_bounds__(TD_THREADS, 2)
+tree_decode_paged_kernel(const __grid_constant__ TreeDecodeParams p) {
+  td_decode_body<D, KV_KIND, true, MULTI, true>(p);
+}
+
+template <bool MULTI>
+const void* pick_td_paged(int d, int kv_kind) {
+  if (d == 128) {
+    if (kv_kind == 0) return (const void*)tree_decode_paged_kernel<128, 0, MULTI>;
+    if (kv_kind == 1) return (const void*)tree_decode_paged_kernel<128, 1, MULTI>;
+    return (const void*)tree_decode_paged_kernel<128, 2, MULTI>;
+  }
+  if (kv_kind == 0) return (const void*)tree_decode_paged_kernel<64, 0, MULTI>;
+  if (kv_kind == 1) return (const void*)tree_decode_paged_kernel<64, 1, MULTI>;
+  return (const void*)tree_decode_paged_kernel<64, 2, MULTI>;
+}
+
 template <bool RANGED, bool MULTI = false>
 const void* pick_td(int d, int kv_kind) {
   if (d == 128) {
@@ -410,17 +449,21 @@ const void* pick_td(int d, int kv_kind) {
 
 }  // namespace
 
-int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged, bool multi) {
+int tree_decode_max_ctas(int d, int kv_kind, int num_sms, bool ranged, bool multi, bool paged) {
   int per_sm = 0;
-  const void* fn = multi ? pick_td<true, true>(d, kv_kind)
+  const void* fn = paged ? (multi ? pick_td_paged<true>(d, kv_kind) : pick_td_paged<false>(d, kv_kind))
+                 : multi ? pick_td<true, true>(d, kv_kind)
                          : (ranged ? pick_td<true>(d, kv_kind) : pick_td<false>(d, kv_kind));
   cuda_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, TD_THREADS, 0), "tree_decode occupancy");
   return per_sm * num_sms;
 }
 
 void launch_tree_decode(const TreeDecodeParams& p, int d, int grid, cudaStream_t stream, bool ranged) {
-  const void* fn = p.tokens > 1 ? pick_td<true, true>(d, p.kv_kind)
-                                : (ranged ? pick_td<true>(d, p.kv_kind) : pick_td<false>(d, p.kv_kind));
+  const bool multi = p.tokens > 1;
+  const void* fn = p.block_table != nullptr
+                       ? (multi ? pick_td_paged<true>(d, p.kv_kind) : pick_td_paged<false>(d, p.kv_kind))
+                   : multi ? pick_td<true, true>(d, p.kv_kind)
+                           : (ranged ? pick_td<true>(d, p.kv_kind) : pick_td<false>(d, p.kv_kind));
   void* args[] = {(void*)&p};
   // cooperative: the grid barrier and the cross-rank waits need every CTA of the grid to be resident
   cuda_check(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(TD_THREADS), args, 0, stream), "tree_decode launch");

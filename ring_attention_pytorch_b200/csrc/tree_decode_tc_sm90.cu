@@ -93,12 +93,15 @@ __device__ __forceinline__ void widen_fp8_tile(const uint8_t* src, uint8_t* dst,
 // and softclamp (TreeDecodeParams); V rows of invisible keys in a unit's boundary tiles are zeroed in shared memory,
 // since a probability of 0 does not cancel a NaN value row inside the MMA.  MULTI (with RANGED): the columns are the
 // (query head, token) pairs of a multi-token call; the unit streams the union of its tokens' key ranges and, in the
-// tiles that cross some column's bounds, masks each (key, column) with that column's range.
-template <int KVK, int NH, bool RANGED, bool MULTI = false>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
-                      const __grid_constant__ TreeDecodeParams p) {
+// tiles that cross some column's bounds, masks each (key, column) with that column's range.  PAGED (with RANGED): K / V
+// come from page pools through 4-D tensor maps (d, page_size, hk, num_pages), one box of min(page_size, 64) keys per
+// page run of a sub-tile; each box's first key is clamped into [lo, k1 - 1] before its page id is read, so only table
+// entries of visible pages are dereferenced (the boxes that clamp away are masked like any key outside the range).
+template <int KVK, int NH, bool RANGED, bool MULTI, bool PAGED>
+__device__ __forceinline__ void tc_decode_body(const CUtensorMap& map_k, const CUtensorMap& map_v,
+                                               const TreeDecodeParams& p) {
   static_assert(RANGED || !MULTI, "a multi-token call takes the ranged body");
+  static_assert(RANGED || !PAGED, "a paged call takes the ranged body");
   constexpr bool KV8 = KVK == 2;
   constexpr bool F16 = KVK == 1;
   constexpr int D = TC_D;
@@ -184,11 +187,39 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
     const float* ksb = p.k_scale ? p.k_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
     const float* vsb = p.v_scale ? p.v_scale + (size_t)bhk * p.n_scale_blocks : nullptr;
 
+    // paged: the (page, slot) of each box of the next tile to issue.  Thread 0 reads them one tile ahead of the issue,
+    // so the table load is in flight during a tile of compute instead of in front of the TMA.
+    const int box_keys = PAGED ? min(p.page_size, TC_TILE) : TC_TILE;
+    const int nbox = TC_TILE / box_keys;
+    int pg[4], sl[4];
+    auto lookup = [&](int i) {
+      const int* tbl = p.block_table + (size_t)b * p.max_pages;
+#pragma unroll
+      for (int x = 0; x < 4; ++x) {
+        if (x < nbox) {
+          const int key = min(max(k0 + i * TC_TILE + x * box_keys, lo), k1 - 1);
+          pg[x] = __ldg(tbl + key / p.page_size);
+          sl[x] = (key % p.page_size) & ~(box_keys - 1);
+        }
+      }
+    };
     auto issue = [&](int i) {  // tile i of this unit into stage (n_tile + i) % TC_NST
       const uint32_t st = (n_tile + i) % TC_NST;
       const int key0 = k0 + i * TC_TILE;
       mbar_expect_tx(&sm.full[st], TX);
-      if constexpr (KV8) {
+      if constexpr (PAGED) {
+#pragma unroll
+        for (int s = 0; s < (KV8 ? 1 : 2); ++s) {
+#pragma unroll
+          for (int x = 0; x < 4; ++x) {
+            if (x < nbox) {  // each box lands 1 KB aligned: the sub-tile's 128B swizzle pattern is unchanged
+              const int off = s * TC_SUB + x * box_keys * 128;
+              tma_load_4d(sm.k[st] + off, &map_k, &sm.full[st], s * 64, sl[x], kvh, pg[x]);
+              tma_load_4d(sm.v[st] + off, &map_v, &sm.full[st], s * 64, sl[x], kvh, pg[x]);
+            }
+          }
+        }
+      } else if constexpr (KV8) {
         tma_load_3d(sm.k[st], &map_k, &sm.full[st], 0, key0, bhk);
         tma_load_3d(sm.v[st], &map_v, &sm.full[st], 0, key0, bhk);
       } else {
@@ -199,8 +230,15 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
         }
       }
     };
-    if (tid == 0)
-      for (int i = 0; i < min(TC_NST, ntiles); ++i) issue(i);
+    if (tid == 0) {
+      for (int i = 0; i < min(TC_NST, ntiles); ++i) {
+        if constexpr (PAGED) lookup(i);
+        issue(i);
+      }
+      if constexpr (PAGED) {
+        if (TC_NST < ntiles) lookup(TC_NST);
+      }
+    }
 
     // Q^T as the B operand (16 bit, zero for padded heads); the softmax scale is applied to the logits
     for (int i = tid; i < ((!RANGED || ntiles > 0) ? NH * D / 2 : 0); i += TC_THREADS) {
@@ -348,7 +386,12 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
       fence_regs(o[0]);
       fence_regs(o[1]);
       named_bar_sync(1, TC_THREADS);  // every warp is done with stage st, the widened tiles and P
-      if (tid == 0 && t + TC_NST < ntiles) issue(t + TC_NST);
+      if (tid == 0 && t + TC_NST < ntiles) {
+        issue(t + TC_NST);
+        if constexpr (PAGED) {
+          if (t + TC_NST + 1 < ntiles) lookup(t + TC_NST + 1);
+        }
+      }
     }
     n_tile += ntiles;
 
@@ -438,6 +481,21 @@ tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_co
   td_cross_rank_merge<D, MULTI>(p, cs, total_units);
 }
 
+template <int KVK, int NH, bool RANGED, bool MULTI = false>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tree_decode_tc_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                      const __grid_constant__ TreeDecodeParams p) {
+  tc_decode_body<KVK, NH, RANGED, MULTI, false>(map_k, map_v, p);
+}
+
+// paged K / V (TreeDecodeParams::block_table): always the ranged body
+template <int KVK, int NH, bool MULTI>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tree_decode_tc_paged_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                            const __grid_constant__ TreeDecodeParams p) {
+  tc_decode_body<KVK, NH, true, MULTI, true>(map_k, map_v, p);
+}
+
 template <int KVK, bool RANGED>
 const void* tc_ptr_nh(bool small_group) {
   return small_group ? (const void*)tree_decode_tc_kernel<KVK, 8, RANGED>
@@ -469,6 +527,21 @@ const void* pick_tc_r(int kv_kind, bool small_group) {
 const void* pick_tc(int kv_kind, bool small_group, bool ranged) {
   return ranged ? pick_tc_r<true>(kv_kind, small_group) : pick_tc_r<false>(kv_kind, small_group);
 }
+// paged calls: NH = 8 or 16 single-token (small_group), 8, 16 or 32 multi-token (tc_multi_nh)
+template <int KVK>
+const void* tc_ptr_paged(bool multi, int nh) {
+  if (multi) {
+    if (nh == 8) return (const void*)tree_decode_tc_paged_kernel<KVK, 8, true>;
+    if (nh == 16) return (const void*)tree_decode_tc_paged_kernel<KVK, 16, true>;
+    return (const void*)tree_decode_tc_paged_kernel<KVK, 32, true>;
+  }
+  return nh == 8 ? (const void*)tree_decode_tc_paged_kernel<KVK, 8, false>
+                 : (const void*)tree_decode_tc_paged_kernel<KVK, 16, false>;
+}
+const void* pick_tc_paged(int kv_kind, bool multi, int nh) {
+  if (kv_kind == 2) return tc_ptr_paged<2>(multi, nh);
+  return kv_kind == 1 ? tc_ptr_paged<1>(multi, nh) : tc_ptr_paged<0>(multi, nh);
+}
 size_t tc_smem(int kv_kind, bool small_group) {
   size_t s;
   if (kv_kind == 2) s = small_group ? sizeof(TcSmem<true, 8>) : sizeof(TcSmem<true, 16>);
@@ -478,11 +551,12 @@ size_t tc_smem(int kv_kind, bool small_group) {
 
 }  // namespace
 
-int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged, int cols) {
+int tree_decode_tc_max_ctas(int kv_kind, int num_sms, bool ranged, int cols, bool paged) {
   const bool small = false;  // the 16-head variant: the larger shared-memory footprint bounds residency
-  // a multi-token call plans with the residency of the variant it launches
+  // a multi-token or paged call plans with the residency of the variant it launches
   const int nh = tc_multi_nh(cols);
-  const void* fn = cols > 0 ? pick_tc_multi(kv_kind, nh) : pick_tc(kv_kind, small, ranged);
+  const void* fn = paged ? pick_tc_paged(kv_kind, cols > 0, cols > 0 ? nh : 16)
+                         : (cols > 0 ? pick_tc_multi(kv_kind, nh) : pick_tc(kv_kind, small, ranged));
   const size_t smem = cols > 0 ? (kv_kind == 2 ? tc_smem_multi<true>(nh) : tc_smem_multi<false>(nh))
                                : tc_smem(kv_kind, small);
   cuda_check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tree_decode_tc smem attr");
@@ -496,7 +570,8 @@ void launch_tree_decode_tc(const CUtensorMap& map_k, const CUtensorMap& map_v, c
   const bool small = p.heads / p.kv_heads <= 8;
   const bool multi = p.tokens > 1;
   const int nh = tc_multi_nh(p.heads / p.kv_heads * p.tokens);
-  const void* fn = multi ? pick_tc_multi(p.kv_kind, nh) : pick_tc(p.kv_kind, small, ranged);
+  const void* fn = p.block_table != nullptr ? pick_tc_paged(p.kv_kind, multi, multi ? nh : (small ? 8 : 16))
+                   : (multi ? pick_tc_multi(p.kv_kind, nh) : pick_tc(p.kv_kind, small, ranged));
   const size_t smem = multi ? (p.kv_kind == 2 ? tc_smem_multi<true>(nh) : tc_smem_multi<false>(nh))
                             : tc_smem(p.kv_kind, small);
   cuda_check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tree_decode_tc smem attr");

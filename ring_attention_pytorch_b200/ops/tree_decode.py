@@ -23,7 +23,9 @@ import torch.distributed as dist
 from torch import Tensor
 
 from ring_attention_pytorch_b200.parallel.distributed import default, exists, get_rank, get_world_size, is_distributed
-from ring_attention_pytorch_b200.utils.validate import check_decode_query, check_decode_ranges, check_sinks, typecheck
+from ring_attention_pytorch_b200.ops.paged_kv import gather_paged_kv
+from ring_attention_pytorch_b200.utils.validate import (check_decode_query, check_decode_ranges, check_paged_kv, check_sinks,
+                                                         typecheck)
 
 
 def _visible_keys(n: int, cache_seqlens: Optional[Tensor], q_pos: Optional[Tensor], window: Optional[int],
@@ -84,6 +86,7 @@ def tree_attn_decode(
     window: Optional[int] = None,
     softclamp_value: float = 0.0,
     kv_pos: Optional[tuple[int, int]] = None,
+    block_table: Optional[Tensor] = None,
 ) -> Tensor:
     """``q [b, h, m, d]``; returns ``[b, h, m, dv]`` in ``q.dtype``.
 
@@ -109,6 +112,14 @@ def tree_attn_decode(
     among themselves.  The caller appends the tokens' K/V first and counts them in ``cache_seqlens``.  Without
     ``q_pos`` there is no position rule and every token sees every held key -- speculative verification needs
     ``q_pos``.  GQA, softclamp, sinks (once per token row) and the cache formats apply per token row.
+
+    Paged KV cache: with ``block_table`` (int32 ``[b, max_pages]``) ``k`` / ``v`` are this rank's page pools
+    ``[num_pages, hk, page_size, d]`` (or an NHD pool passed as ``.transpose(1, 2)``), and local key ``j`` of sequence
+    ``b`` is ``pool[block_table[b, j // page_size], :, j % page_size]``: the call equals the one on
+    ``gather_paged_kv(pool, block_table)`` (``ops/paged_kv.py``).  It needs ``shard_kv_seq=False`` (each rank passes
+    its own pools, table, ``cache_seqlens`` and ``kv_pos``) and ``cache_seqlens``; ``page_size`` is 16, 32 or a
+    multiple of 64.  Entries of pages that hold no key visible to any token of the call are never read (they may name a
+    freed page); entries are not checked and must lie in ``[0, num_pages)``.
     """
     assert not (exists(k) ^ exists(v)), "keys and values are either both None, or both present"
     check_decode_query(q, name="tree_attn_decode")
@@ -116,6 +127,10 @@ def tree_attn_decode(
     b, h, m = q.shape[:3]
     check_sinks(sinks, h, q.device, name="tree_attn_decode")
     check_decode_ranges(b, q.device, cache_seqlens, q_pos, window, kv_pos, softclamp_value, name="tree_attn_decode")
+    if exists(block_table) and shard_kv_seq:
+        raise ValueError("tree_attn_decode: a paged cache (block_table) needs shard_kv_seq=False: each rank passes its "
+                         "own page pools and table")
+    check_paged_kv(b, q.device, k, v, block_table, cache_seqlens, name="tree_attn_decode")
     ranged = exists(cache_seqlens) or exists(q_pos) or softclamp_value > 0
     if exists(v):
         dim_v = v.shape[-1]
@@ -146,9 +161,12 @@ def tree_attn_decode(
 
         if ranged:
             return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps, sinks=sinks, cache_seqlens=cache_seqlens, q_pos=q_pos,
-                                    window=window, kv_pos=kv_pos, softclamp_value=softclamp_value).to(dtype)
+                                    window=window, kv_pos=kv_pos, softclamp_value=softclamp_value,
+                                    block_table=block_table).to(dtype)
         return tree_decode_cuda(q, k, v, dim_v=dim_v, eps=eps, sinks=sinks).to(dtype)
 
+    if exists(block_table):
+        k, v = gather_paged_kv(k, block_table), gather_paged_kv(v, block_table)
     if exists(k) and k.shape[-2] > 0 and ranged:
         visible = _visible_keys(k.shape[-2], cache_seqlens, q_pos, window, kv_pos, b, q.device, m)
         local_out, lse = _local_attention(q, k, v, visible, softclamp_value)

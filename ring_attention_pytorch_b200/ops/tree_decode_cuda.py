@@ -19,7 +19,7 @@ from torch import Tensor
 
 from ring_attention_pytorch_b200.ops import _ext
 from ring_attention_pytorch_b200.parallel.distributed import get_rank, get_world_size, is_distributed
-from ring_attention_pytorch_b200.utils.validate import check_decode_query, check_decode_ranges
+from ring_attention_pytorch_b200.utils.validate import check_decode_query, check_decode_ranges, check_paged_kv
 
 LAUNCHES = {"count": 0}
 # nvls "auto": use the NVSwitch multicast mapping when torch's symmetric memory can provide one, else NVLink peer loads
@@ -58,12 +58,15 @@ def decode_span(n: int, window: Optional[int] = None, kv_pos_stride: int = 1, to
 
 
 def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int, *, ranged: bool = False,
-                span: Optional[int] = None, tokens: int = 1) -> DecodePlan:
+                span: Optional[int] = None, tokens: int = 1, paged: bool = False) -> DecodePlan:
     """The kernel and the work split a decode call of these sizes gets (``kv_kind``: 0 bf16, 1 fp16, 2 fp8 cache).
     ``ranged``: the instantiations with per-sequence key ranges / softclamp; ``span`` (default ``n``): the keys the
     splits are planned over (:func:`decode_span`).  ``tokens > 1``: a multi-token call (always ranged), whose work
     units hold ``NH`` (query head, token) columns of one kv head -- 8, 16 or 32 for ``g * tokens`` up to 8, up to 16,
-    larger on the tensor-core kernel, 4 on the CUDA-core kernel -- planned with that variant's residency."""
+    larger on the tensor-core kernel, 4 on the CUDA-core kernel -- planned with that variant's residency.
+    ``paged`` (always ranged; ``n = max_pages * page_size``): the splits are those of a contiguous cache of ``n`` keys,
+    so the paged call computes bitwise what that call computes; the grid is bounded by the paged variant's residency."""
+    assert ranged or tokens > 1 or not paged, "a paged call is ranged"
     tc = CONFIG["tensor_core"]
     use_tc = tc in ("auto", True, "on") and d == 128 and n >= 1
     g = h // hk
@@ -72,7 +75,10 @@ def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int, *, ranged
         gm = (8 if cols <= 8 else (16 if cols <= 16 else 32)) if use_tc else 4
         groups = b * hk * ((cols + gm - 1) // gm)
         resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc, True, cols))
-        return DecodePlan(use_tc, groups, resident, _choose_splits(n if span is None else span, groups, resident))
+        splits = _choose_splits(n if span is None else span, groups, resident)
+        if paged:
+            resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc, True, cols, True))
+        return DecodePlan(use_tc, groups, resident, splits)
     gm = (8 if g <= 8 else 16) if use_tc else 4  # query heads per work unit (tensor-core kernel: MMA N)
     groups = b * hk * ((g + gm - 1) // gm)
     resident = int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc))
@@ -80,7 +86,8 @@ def decode_plan(b: int, h: int, hk: int, n: int, d: int, kv_kind: int, *, ranged
         # the splits follow the plain kernel's residency, so full-length ranges split exactly like the plain call;
         # the grid is bounded by the ranged kernel's own residency (cooperative launch)
         splits = _choose_splits(n if span is None else span, groups, resident)
-        return DecodePlan(use_tc, groups, int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc, True)), splits)
+        return DecodePlan(use_tc, groups, int(_ext.ops().tree_decode_max_ctas(d, kv_kind, use_tc, True, 0, paged)),
+                          splits)
     return DecodePlan(use_tc, groups, resident, _choose_splits(n, groups, resident))
 
 
@@ -200,6 +207,7 @@ def tree_decode_cuda(
     window: Optional[int] = None,
     kv_pos: Tuple[int, int] = (0, 1),
     softclamp_value: float = 0.0,
+    block_table: Optional[Tensor] = None,
 ) -> Tensor:
     """q [b, h, m, d] (bf16 / fp16 / fp32; m >= 1 query tokens per sequence); k, v [b, hk, n, d] this rank's shard
     (bf16 / fp16 / float8_e4m3fn) or None.
@@ -223,12 +231,23 @@ def tree_decode_cuda(
     each token applies the rule above at its own position, so the tokens are causal among themselves; their K / V are
     appended (and counted in ``cache_seqlens``) before the call.  Without ``q_pos`` there is no position rule: every
     token sees every held key.  One pass over the cache serves all ``m`` tokens.  ``q_pos + m - 1`` must fit in int32.
+
+    Paged KV cache (``block_table``, int32 ``[b, max_pages]``, contiguous for an allocation-free call): ``k`` / ``v``
+    are page pools ``[num_pages, hk, page_size, d]`` (an NHD pool ``[num_pages, page_size, hk, d]`` passed as
+    ``.transpose(1, 2)`` works too) and local key ``j`` of sequence ``b`` is ``pool[block_table[b, j // page_size], :,
+    j % page_size]``.  The call computes exactly the contiguous call on ``gather_paged_kv(pool, block_table)``
+    (``ops/paged_kv.py``), ``n = max_pages * page_size``, with every rule above.  ``cache_seqlens`` is required;
+    ``page_size`` is 16, 32 or a multiple of 64.  Table entries of pages that hold no key visible to a token of the
+    call are never read, so they may point at any page (e.g. one freed behind a window and reused).  Entries are not
+    checked (that would need a host sync) and must lie in ``[0, num_pages)``.
     """
     check_decode_query(q, out, dim_v, name="tree_decode_cuda")
-    ops = _ext.ops()
     b, h, m, d = q.shape
     check_decode_ranges(b, q.device, cache_seqlens, q_pos, window, kv_pos, softclamp_value, name="tree_decode_cuda")
-    ranged = cache_seqlens is not None or q_pos is not None or softclamp_value > 0 or m > 1
+    check_paged_kv(b, q.device, k, v, block_table, cache_seqlens, name="tree_decode_cuda")
+    ops = _ext.ops()
+    paged = block_table is not None and block_table.shape[1] > 0
+    ranged = cache_seqlens is not None or q_pos is not None or softclamp_value > 0 or m > 1 or paged
     assert dim_v == d, "the decode kernel assumes dim_v == dim_qk"
     dev = q.device
     q3 = q.reshape(b, h, d) if m == 1 else q
@@ -237,7 +256,14 @@ def tree_decode_cuda(
     if q3.dtype not in (torch.bfloat16, torch.float16, torch.float32):
         q3 = q3.float()
     n, hk = 0, h
-    if k is not None and k.shape[-2] > 0:
+    if paged:
+        if k.dtype == torch.float32:
+            k, v = k.to(torch.bfloat16), v.to(torch.bfloat16)
+        hk, n = k.shape[1], block_table.shape[1] * k.shape[2]
+        block_table = block_table.contiguous()
+    elif block_table is not None:  # no pages: this rank holds no keys
+        k = v = None
+    elif k is not None and k.shape[-2] > 0:
         if k.dtype == torch.float32:
             k, v = k.to(torch.bfloat16), v.to(torch.bfloat16)
         hk, n = k.shape[1], k.shape[2]
@@ -247,13 +273,14 @@ def tree_decode_cuda(
     kv_kind = 0 if k is None or k.dtype == torch.bfloat16 else (1 if k.dtype == torch.float16 else 2)
     if m > 1:
         plan = decode_plan(b, h, hk, n, d, kv_kind, ranged=True, span=decode_span(n, window, int(kv_pos[1]), m),
-                           tokens=m)
+                           tokens=m, paged=paged)
     elif ranged:
-        plan = decode_plan(b, h, hk, n, d, kv_kind, ranged=True, span=decode_span(n, window, int(kv_pos[1])))
+        plan = decode_plan(b, h, hk, n, d, kv_kind, ranged=True, span=decode_span(n, window, int(kv_pos[1])),
+                           paged=paged)
     else:
         plan = decode_plan(b, h, hk, n, d, kv_kind)
     use_tc, groups, resident, splits = plan.tensor_core, plan.groups, plan.resident, plan.splits
-    if k is not None and not (use_tc and _is_cache_prefix(k) and v.stride() == k.stride()):
+    if k is not None and not paged and not (use_tc and _is_cache_prefix(k) and v.stride() == k.stride()):
         k, v = k.contiguous(), v.contiguous()  # no-op for dense inputs
     buf = _buffers(b * h * m, d, dev)
     need = b * hk * splits * g * m * (d + 4)  # scratch rows: (b, kv head, split, column), g * m columns
@@ -277,7 +304,7 @@ def tree_decode_cuda(
                         hk, splits, d ** -0.5, scale_block_keys, eps, grid, use_tc, sinks,
                         cache_seqlens.contiguous() if cache_seqlens is not None else None, q_pos.contiguous()
                         if q_pos is not None else None, window or 0, int(kv_pos[0]), int(kv_pos[1]),
-                        float(softclamp_value))
+                        float(softclamp_value), block_table if paged else None)
     else:
         ops.tree_decode(q3, k, v, k_scale, v_scale, buf.scratch, buf.group_done, buf.counters, buf.partial_ptrs,
                         buf.aux_local_ptr, buf.pad_ptrs, buf.mc_partial_ptr, buf.mc_aux_ptr, buf.rank, out_k,

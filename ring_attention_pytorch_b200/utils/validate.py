@@ -114,6 +114,42 @@ def check_decode_ranges(batch: int, device, cache_seqlens: Optional[Tensor], q_p
         raise ValueError(f"{name}: softclamp_value must be >= 0, got {softclamp_value}")
 
 
+def check_paged_kv(batch: int, device, k, v, block_table: Optional[Tensor], cache_seqlens: Optional[Tensor], *,
+                   name: str = "decode") -> None:
+    """A paged decode call: ``block_table`` int32 ``[batch, max_pages]`` on the inputs' device, ``cache_seqlens``
+    given, and ``k`` / ``v`` page pools ``[num_pages, hk, page_size, d]`` of one shape, dtype and strides, with unit
+    ``d`` stride, strides that are multiples of 16 bytes, ``page_size`` 16, 32 or a multiple of 64 and
+    ``max_pages * page_size < 2**31``.  The table's entries are not read (no host sync); they must lie in
+    ``[0, num_pages)``."""
+    if block_table is None:
+        return
+    if not torch.is_tensor(block_table) or block_table.dim() != 2 or block_table.shape[0] != batch:
+        raise ValueError(f"{name}: block_table must be a 2-D tensor [batch = {batch}, max_pages], got "
+                         f"{tuple(block_table.shape) if torch.is_tensor(block_table) else type(block_table)}")
+    if block_table.dtype != torch.int32:
+        raise ValueError(f"{name}: block_table must be int32, got {block_table.dtype}")
+    if block_table.device != torch.device(device):
+        raise ValueError(f"{name}: block_table must live on {device}, got {block_table.device}")
+    if cache_seqlens is None:
+        raise ValueError(f"{name}: a paged cache (block_table) needs cache_seqlens, the keys held by each sequence")
+    if not torch.is_tensor(k) or not torch.is_tensor(v):
+        raise ValueError(f"{name}: block_table needs the k and v page pools")
+    if k.dim() != 4 or k.shape != v.shape or k.dtype != v.dtype or k.stride() != v.stride():
+        raise ValueError(f"{name}: the k and v page pools [num_pages, hk, page_size, d] must share shape, dtype and "
+                         f"strides, got {k.dtype} {tuple(k.shape)} {k.stride()} and {v.dtype} {tuple(v.shape)} "
+                         f"{v.stride()}")
+    if k.stride(3) != 1:
+        raise ValueError(f"{name}: the page pools need unit stride on the head dim, got strides {k.stride()}")
+    ps = k.shape[2]
+    if ps not in (16, 32) and not (ps > 0 and ps % 64 == 0):
+        raise ValueError(f"{name}: page_size (pool dim 2) must be 16, 32 or a multiple of 64, got {ps}")
+    if any(s * k.element_size() % 16 for s in k.stride()[:3]):
+        raise ValueError(f"{name}: the page pools' strides must be multiples of 16 bytes, got {k.stride()} elements "
+                         f"of {k.element_size()} bytes")
+    if block_table.shape[1] * ps >= 2 ** 31:
+        raise ValueError(f"{name}: max_pages * page_size must be below 2**31, got {block_table.shape[1]} * {ps}")
+
+
 def check_fp8_attention_inputs(q: Tensor, k: Tensor, v: Tensor, q_descale, k_descale, v_descale,
                                mask: Optional[Tensor] = None, *, name: str = "attention",
                                rotary_freqs: Optional[Tensor] = None, sinks: Optional[Tensor] = None) -> None:
